@@ -1,7 +1,7 @@
 #!/usr/bin/env python
 """bench.py -- hot-path benchmark (contract in the task statement, section 4).
 
-  python bench.py [--gpus N] [--steps K] [--warmup W] [--impl ours|reference] [--workload NAME]
+  python bench.py [--gpus N] [--steps K] [--warmup W] [--impl ours|reference] [--workload NAME] [--dump-outputs DIR]
   python -m torch.distributed.run --nnodes=1 --nproc-per-node N ... bench.py --gpus N ...
 
 A *step* is one pass of the NLMeans hot path over one batch of `--batch` synthetic frames per GPU, taken from ONE
@@ -10,21 +10,24 @@ restarts between steps, so no step pays a pipeline fill or an EOF flush).  With 
 frames) both timed regions last seconds, not milliseconds.
 
   value     frames/s, whole job, inputs already resident in HBM (border + NLMeans kernels, CUDA events on the
-            compute streams; the step's inputs cycle through 32 distinct device frames = 398 MB > 126 MB L2)
+            compute streams; the step's inputs cycle through 32 distinct device frames = 398 MB > 50 MB L2)
   e2e       frames/s through hb_filter_nlmeans_cuda.work() with HOST hb_buffer_t frames: pinned H2D + kernels +
             D2H into fresh output buffers, all inside the timed region (hb_bench.c: decoder-style input buffers
             over a bounded ring of pinned payloads)
   roofline  algorithmic HBM bytes of the NLMeans kernel (3 x frame bytes per output frame, SURVEY.md 8d) / its
-            CUDA-event time, against MEASURED_PEAKS.json; issue_frac = warp instructions of one launch (committed
-            ncu capture) / (148 SMs x 4 schedulers x clock x kernel time) -- the roofline this kernel actually sits under
+            CUDA-event time, against MEASURED_PEAKS.json (else the H100 SXM data sheet's 3.35 TB/s)
   cpu_baseline / --impl reference
-            the reference's own nlmeans.c + nlmeans_x86.c (oracle/_ref/libhbref.so, compiled unmodified from
-            /root/reference) on this box's host cores, same frames, same protocol, one continuous stream
+            the reference's own nlmeans.c + nlmeans_x86.c (oracle/_ref/libhbref.so, compiled unmodified where the
+            HandBrake sources were present at build time; reported as not run otherwise) on this box's host cores,
+            same frames, same protocol, one continuous stream
   extra     (N = 1) the other BASELINE.json configurations, each with e2e / cpu_baseline / roofline:
             config 2 (1080p NLMeans medium), config 3 (4K 10-bit comb-detect + decomb EEDI2 bob), config 4 with the
             large search window (patch 5, range 7, frames 4), config 5 (8K 10-bit chain, frames device-resident
             between the filters)
   copy_only the e2e pipeline with every plane bypassed: the transfer ceiling of this box at this N
+
+--dump-outputs DIR writes, after the timed steps, the last frame the timed (kernel-only) arm filtered in its last step:
+DIR/y.npy, u.npy, v.npy as float32 planes.  With the same arguments the inputs are the same from run to run.
 """
 import argparse
 import ctypes as C
@@ -42,11 +45,15 @@ import numpy as np
 
 REPO = Path(__file__).resolve().parent
 sys.path.insert(0, str(REPO))
+REF_SO = REPO / "oracle" / "_ref" / "libhbref.so"           # the reference's filters, for the CPU baseline
+# what cpu_baseline says where build() found no HandBrake tree to build the reference's filters from (oracle/Makefile)
+NO_REF = {"value": None, "note": "not run: oracle/_ref/libhbref.so (the reference's filters) is missing; __graft_entry__.build() "
+                                 "builds it where the HandBrake sources are (oracle/Makefile REF, or HANDBRAKE_SRC)"}
 
 from handbrake_b200 import synth  # noqa: E402
 
 WORKLOADS = {
-    # BASELINE.json configs[3]: the configuration the metric ("4K NLMeans frames/sec at 1/2/4/8 B200") is quoted on
+    # BASELINE.json configs[3]: the configuration the metric ("4K NLMeans frames/sec at 1/2/4/8 GPUs") is quoted on
     "4k_nlmeans_strong": dict(width=3840, height=2160, depth=8, settings="y-strength=10", nframes=2,
                               desc="3840x2160 yuv420p 8-bit, NLMeans 'strong' (strength 10, patch 7, range 3, frames 2)"),
     "4k_nlmeans_medium": dict(width=3840, height=2160, depth=8, settings="y-strength=6", nframes=2,
@@ -153,7 +160,7 @@ def open_chain(lib, names, settings, fmt, w, h, flags):
 
 
 class ClockSampler:
-    """nvidia-smi clocks / throttle reasons during the timed region (B200_PROFILING.md recipe)"""
+    """nvidia-smi clocks / throttle reasons during the timed region"""
     Q = "clocks.sm,clocks.max.sm,power.draw,clocks_event_reasons.hw_slowdown,clocks_event_reasons.hw_thermal_slowdown," \
         "clocks_event_reasons.sw_thermal_slowdown,clocks_event_reasons.sw_power_cap"
 
@@ -206,8 +213,8 @@ class ClockSampler:
 def measured_peaks():
     p = REPO / "MEASURED_PEAKS.json"
     if p.exists():
-        return json.loads(p.read_text()).get("hbm_gbs", 6650.0), "measured (MEASURED_PEAKS.json)"
-    return 6650.0, "fallback (B200_PROFILING.md)"
+        return json.loads(p.read_text()).get("hbm_gbs", 3350.0), "measured (MEASURED_PEAKS.json)"
+    return 3350.0, "H100 SXM data sheet (HBM3, 3.35 TB/s)"
 
 
 def gpu_numa_cpus(gpu_index):
@@ -318,18 +325,6 @@ def plane_ptrs(t, dims, bps):
     return (C.c_void_p * 3)(*ptrs), (C.c_int * 3)(*strides)
 
 
-def ncu_capture(workload, depth):
-    """numbers of the committed `ncu --set full` capture of this workload's kernel (never measured live: a run under
-    ncu is not a bench value)"""
-    names = {("4k_nlmeans_strong", 8): ["r02_nlmeans_v3_ncu.json", "r01g_nlmeans_fused_ncu.json"],
-             ("4k10_nlmeans_medium", 10): ["r02_nlmeans_v3w_ncu.json"]}
-    for n in names.get((workload, depth), []):
-        p = REPO / "profiles" / n
-        if p.exists():
-            return json.loads(p.read_text()), f"profiles/{n}"
-    return None, None
-
-
 class Ours:
     """the CUDA libraries + torch, bound once per process"""
 
@@ -355,15 +350,16 @@ class Ours:
         if rc != 0:
             raise RuntimeError(self.core.hbcu_last_error().decode())
 
-    def nlmeans_device_arm(self, wl, host, B, K, Wm, barrier=lambda: None, clock=None):
+    def nlmeans_device_arm(self, wl, host, B, K, Wm, barrier=lambda: None, clock=None, dump=None):
         """kernel-only arm: one continuous stream whose raw frames are already in HBM.  Frame t+nf-1 is bordered
-        (upload_device) just before frame t is filtered, like the filter object does.  Returns (ms, kernel stats)."""
+        (upload_device) just before frame t is filtered, like the filter object does.  Returns (ms, kernel stats).
+        dump: a directory to write the last frame of the last timed step to (float32 planes y, u, v)."""
         torch, core, ck = self.torch, self.core, self.ck
         W, H, depth, nf = wl["width"], wl["height"], wl["depth"], wl["nframes"]
         bps = 2 if depth > 8 else 1
         dims = synth.plane_dims(W, H)
         fb = host.shape[1]
-        n_dev = max(8, min(32, int(420e6 // fb) + 1))                    # distinct device frames: > L2 (126 MB) in total
+        n_dev = max(8, min(32, int(420e6 // fb) + 1))                    # distinct device frames: > L2 (50 MB) in total
         dev = [torch.from_numpy(host[i % host.shape[0]]).cuda() for i in range(n_dev)]
         ptrs = [plane_ptrs(t, dims, bps) for t in dev]
         cfg = nlm_config(self.flt, wl, self.gpu, ring=nf + 6, out_slots=4)
@@ -372,13 +368,15 @@ class Ours:
         state = {"t": 0}
         for i in range(nf - 1):
             ck(core.hbcu_nlmeans_upload_device(h, C.c_int64(i), ptrs[i % n_dev][0], ptrs[i % n_dev][1]))
+        # where filter_device leaves each frame (its output slot): read back for --dump-outputs
+        out_planes, out_strides = (C.c_void_p * 3)(), (C.c_int * 3)()
 
         def step():
             t0 = state["t"]
             for t in range(t0, t0 + B):
                 u = t + nf - 1
                 ck(core.hbcu_nlmeans_upload_device(h, C.c_int64(u), ptrs[u % n_dev][0], ptrs[u % n_dev][1]))
-                ck(core.hbcu_nlmeans_filter_device(h, C.c_int64(t), nf, None, None))
+                ck(core.hbcu_nlmeans_filter_device(h, C.c_int64(t), nf, out_planes, out_strides))
             state["t"] = t0 + B
 
         for _ in range(Wm):
@@ -399,6 +397,8 @@ class Ours:
         barrier()
         kms, kcalls = C.c_float(), C.c_int()
         ck(core.hbcu_nlmeans_kernel_ms(h, C.byref(kms), C.byref(kcalls)))
+        if dump is not None:
+            dump_planes(torch, dump, out_planes, out_strides, dims, bps)
         core.hbcu_nlmeans_destroy(h)
         del dev
         torch.cuda.empty_cache()
@@ -431,7 +431,23 @@ class Ours:
         return res
 
 
-def nlm_roofline(wl, workload, ms, ks, frames, clocks_mhz=None):
+class DevicePlane:
+    """a pitched device plane the filter owns, seen by torch without a copy"""
+
+    def __init__(self, ptr, pitch, w, h, bps):
+        self.__cuda_array_interface__ = {"shape": (h, w), "typestr": "<u2" if bps == 2 else "|u1", "data": (ptr, False),
+                                         "strides": (pitch, bps), "version": 3}
+
+
+def dump_planes(torch, out_dir, planes, strides, dims, bps):
+    out_dir = Path(out_dir)
+    out_dir.mkdir(parents=True, exist_ok=True)
+    for name, ptr, pitch, (w, h) in zip(("y", "u", "v"), planes, strides, dims):
+        a = torch.as_tensor(DevicePlane(ptr, pitch, w, h, bps), device="cuda").cpu().numpy()
+        np.save(out_dir / f"{name}.npy", a.astype(np.float32))
+
+
+def nlm_roofline(wl, ms, ks, frames):
     peak, peak_src = measured_peaks()
     fb = synth.frame_bytes(fmt_of(wl["depth"]), wl["width"], wl["height"])
     alg = (wl["nframes"] + 1) * fb
@@ -441,32 +457,22 @@ def nlm_roofline(wl, workload, ms, ks, frames, clocks_mhz=None):
     in_flight = max(1.0, launch_ms * frames / ms) if ms > 0 else 1.0
     kern_ms = launch_ms / in_flight
     achieved = alg / (kern_ms / 1e3) / 1e9 if ks["kernel_calls"] else None
-    cap, cap_src = ncu_capture(workload, wl["depth"])
-    r = {"bound": "hbm", "achieved": round(achieved, 1) if achieved else None, "peak": peak, "unit": "GB/s",
+    return {"bound": "hbm", "achieved": round(achieved, 1) if achieved else None, "peak": peak, "unit": "GB/s",
          "frac": round(achieved / peak, 4) if achieved else None,
-         "traffic": int(cap["dram_bytes_total"]) if cap else None, "traffic_source": cap_src,
          "kernel": ("nlmeans_v3_kernel" if wl["depth"] == 8 else "nlmeans_v3w_kernel") +
                    " (all tiles of Y, U, V of one frame in one launch)",
          "kernel_ms_per_frame": round(kern_ms, 4), "launch_ms_avg": round(launch_ms, 4), "launches_in_flight": round(in_flight, 2),
          "launches_timed": ks["kernel_calls"], "algorithmic_bytes_per_frame": alg, "peak_source": peak_src,
-         "note": "NLMeans is instruction-issue bound on B200, not HBM bound (DESIGN.md 4.1): frac is the honest HBM fraction, issue_frac the "
-                 "fraction of the instruction-issue roofline (148 SMs x 4 warp-instructions per clock)"}
-    if cap and cap.get("warp_instructions") and clocks_mhz:
-        floor_ms = cap["warp_instructions"] / (148 * 4 * clocks_mhz * 1e6) * 1e3
-        r["issue_frac"] = round(floor_ms / kern_ms, 4)
-        r["issue_floor_ms"] = round(floor_ms, 4)
-        r["warp_instructions_per_launch"] = int(cap["warp_instructions"])
-    return r
+         "note": "NLMeans is integer-ALU / instruction-issue bound, not HBM bound: frac is the algorithmic HBM fraction"}
 
 
 def reference_stream(names, settings, fmt, W, H, flags, host, chunk, budget_s, min_chunks=2, max_chunks=64, warm_chunks=0):
     """the unmodified reference filter(s) (oracle/_ref/libhbref.so) on the host cores: ONE continuous stream fed in
     chunks (a chunk = one full taskset cycle of the multithreaded filters) until the time budget is used; the serial
     EOF flush happens once, after the clock"""
-    so = REPO / "oracle" / "_ref" / "libhbref.so"
-    if not so.exists():
-        raise SystemExit("oracle/_ref/libhbref.so missing: run __graft_entry__.build() where /root/reference exists")
-    ref = C.CDLL(str(so))
+    if not REF_SO.exists():
+        raise RuntimeError("oracle/_ref/libhbref.so missing: __graft_entry__.build() makes it where the HandBrake sources are present")
+    ref = C.CDLL(str(REF_SO))
     bind_bench(ref)
     b = open_chain(ref, names, settings, fmt, W, H, flags)
     st = BenchStats()
@@ -549,17 +555,13 @@ def eedi2_device_arm(ours, ex, host):
     peak, peak_src = measured_peaks()
     fps = n / (ms.value / 1e3)
     ach = 8 * fb * fps / 1e9
-    cap = REPO / "profiles" / "r02_eedi2_dram.json"
-    traffic = json.loads(cap.read_text()) if cap.exists() else None
     return {"value": round(fps, 2), "value_unit": "input frames/s (two EEDI2 fields each), every frame combed", "value_seconds": round(ms.value / 1e3, 3),
             "roofline": {"bound": "hbm", "achieved": round(ach, 1), "peak": peak, "unit": "GB/s", "frac": round(ach / peak, 4),
-                         "traffic": traffic.get("dram_bytes_per_frame") if traffic else None,
-                         "traffic_source": "profiles/r02_eedi2_dram.json" if traffic else None,
                          "algorithmic_bytes_per_frame": 8 * fb, "kernel": "decomb EEDI2 bob: stage kernels of both fields, one CUDA graph per field",
                          "peak_source": peak_src}}
 
 
-def run_extra(ours, ex, budget_cpu_s, with_cpu=True):
+def run_extra(ours, ex, budget_cpu_s, with_cpu=True, no_cpu=None):
     """one entry of `extra`: e2e through the filter objects (device-resident chain between upload and download
     adapters), the reference on the host cores (bounded sample), roofline"""
     W, H, depth = ex["width"], ex["height"], ex["depth"]
@@ -597,14 +599,14 @@ def run_extra(ours, ex, budget_cpu_s, with_cpu=True):
         ms, ks = ours.nlmeans_device_arm(wl, host, B, K, 2)
         out["value"] = round(K * B / (ms / 1e3), 2)
         out["value_seconds"] = round(ms / 1e3, 3)
-        out["roofline"] = nlm_roofline(wl, ex["nlm_workload"], ms, ks, K * B)
+        out["roofline"] = nlm_roofline(wl, ms, ks, K * B)
     elif ex["name"].startswith("cfg3"):
         out.update(eedi2_device_arm(ours, ex, host))
     else:
         ach = ex["alg_f"] * fb * e2e / 1e9
         out["value"] = None
         out["roofline"] = {"bound": "hbm", "achieved": round(ach, 1), "peak": peak, "unit": "GB/s", "frac": round(ach / peak, 4),
-                           "traffic": None, "algorithmic_bytes_per_frame": int(ex["alg_f"] * fb), "peak_source": peak_src,
+                           "algorithmic_bytes_per_frame": int(ex["alg_f"] * fb), "peak_source": peak_src,
                            "basis": "end-to-end rate (host frames in and out; no kernel-only arm for a chain): " + ex.get("alg_note", "")}
     if with_cpu:
         refn = [f"hb_filter_{x}" + ("_mt" if x == "lapsharp" else "") for x in ex["filters"]]
@@ -614,6 +616,8 @@ def run_extra(ours, ex, budget_cpu_s, with_cpu=True):
         out["cpu_baseline"] = {"value": round(c["fps"], 4), "unit": "frames/s", "kind": "reference", "cores": c["ncpu"],
                                "sample": f"{c['frames']} frames in {c['chunks']} chunks of {c['chunk']}, one continuous stream, {c['seconds']:.1f} s",
                                "path": " -> ".join(refn)}
+    elif no_cpu is not None:
+        out["cpu_baseline"] = no_cpu
     return out
 
 
@@ -699,7 +703,8 @@ def run_ours(args, wl, rank, world, local_rank):
 
     # ---------------- value: inputs resident in HBM ----------------
     clk = ClockSampler(gpu)
-    dev_ms_local, ks = ours.nlmeans_device_arm(wl, host, B, K, Wm, barrier=barrier, clock=clk)
+    dev_ms_local, ks = ours.nlmeans_device_arm(wl, host, B, K, Wm, barrier=barrier, clock=clk,
+                                               dump=args.dump_outputs if rank == 0 else None)
     dev_ms = max_over_ranks(dev_ms_local)
     value = world * K * B / (dev_ms / 1e3)
 
@@ -771,14 +776,15 @@ def run_ours(args, wl, rank, world, local_rank):
         "config": {"workload": args.workload, "desc": wl["desc"], "frames_per_step_per_gpu": B,
                    "sharding": f"frame blocks x{world}, {wl['nframes'] - 1}-frame temporal halo per block, no data-path collective",
                    "gpu_of_rank0": gpu, "cpu_affinity": numa_cpus,
-                   "l2": f"inputs cycle through {ks['input_mb']:.0f} MB of distinct device frames > 126 MB L2",
+                   "l2": f"inputs cycle through {ks['input_mb']:.0f} MB of distinct device frames > 50 MB L2",
                    "timed_seconds": {"value": round(dev_ms / 1e3, 3), "e2e": round(e2e_s, 3)}},
         "e2e": {"value": round(e2e, 2), "unit": "frames/s", "h2d_bytes_per_step": int(world * r["bytes_in"] // K),
                 "d2h_bytes_per_step": int(world * r["bytes_out"] // K), "seconds": round(e2e_s, 4), "checksum": r["checksum"],
                 "input_ring": args.ring, "ring_misses": r["ring_misses"], "pinned_numa": pinned_numa},
         "gpu_launches": ks["launches"],
         "clocks": clocks,
-        "roofline": nlm_roofline(wl, args.workload, dev_ms_local, ks, K * B, clocks.get("sm_mhz")),
+        "gpu": torch.cuda.get_device_name(gpu),
+        "roofline": nlm_roofline(wl, dev_ms_local, ks, K * B),
     }
     if copy_only is not None:
         out["copy_only"] = copy_only
@@ -786,15 +792,21 @@ def run_ours(args, wl, rank, world, local_rank):
         out["gather"] = gather
     if plugin_multi is not None:
         out["plugin_multi_device"] = plugin_multi
-    if world == 1 and not args.no_cpu_baseline:
+    with_cpu = not args.no_cpu_baseline and REF_SO.exists()
+    no_cpu = NO_REF if not args.no_cpu_baseline and not REF_SO.exists() else None
+    if world == 1 and no_cpu is not None:
+        print("bench.py: " + NO_REF["note"], file=sys.stderr, flush=True)
+    if world == 1 and with_cpu:
         _, out["cpu_baseline"] = cpu_baseline_nlmeans(wl, budget_s=12.0)
+    elif world == 1 and no_cpu is not None:
+        out["cpu_baseline"] = no_cpu
     if world == 1 and not args.no_extra:
         extra = []
         for ex in EXTRAS:
             if args.only_extra and args.only_extra not in ex["name"]:
                 continue
             try:
-                extra.append(run_extra(ours, ex, budget_cpu_s=8.0, with_cpu=not args.no_cpu_baseline))
+                extra.append(run_extra(ours, ex, budget_cpu_s=8.0, with_cpu=with_cpu, no_cpu=no_cpu))
             except Exception as e:  # an extra must never take the headline line down with it
                 extra.append({"workload": ex["name"], "error": f"{type(e).__name__}: {e}"})
         out["extra"] = extra
@@ -887,6 +899,8 @@ def main():
     ap.add_argument("--plugin-warm", type=int, default=256, help=argparse.SUPPRESS)
     ap.add_argument("--block", type=int, default=8, help="frames per device turn of the plugin's multi-device dealing")
     ap.add_argument("--inflight", type=int, default=6, help="frames in flight in the e2e arm (the filter's `threads` setting)")
+    ap.add_argument("--dump-outputs", default=None, metavar="DIR",
+                    help="write the last frame of the last timed step as DIR/{y,u,v}.npy (float32)")
     args = ap.parse_args()
     if args.warmup < 3 and args.impl == "ours":
         args.warmup = 3                     # timing rule: at least three warm-up steps

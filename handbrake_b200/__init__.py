@@ -1,4 +1,4 @@
-"""handbrake_b200 -- B200-native (sm_100a) implementation of libhb's per-pixel
+"""handbrake_b200 -- H100-native (sm_90a) implementation of libhb's per-pixel
 video-filter hot path (NLMeans, comb-detect, decomb/EEDI2, lapsharp) behind
 libhb's own filter plugin interface.
 

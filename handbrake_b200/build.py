@@ -1,6 +1,6 @@
 """Builds the native pieces in-tree (no JIT cache: the .so files travel with the repo).
 
-  lib/libhbcu.so          CUDA kernels + C-ABI (include/hbcu.h), nvcc, sm_100a only
+  lib/libhbcu.so          CUDA kernels + C-ABI (include/hbcu.h), nvcc, sm_90a only
   lib/libhbcu_filters.so  the product's host side: the hb_filter_*_cuda objects in C (gcc) and their libhb-facing
                           helpers, linked against libhbcu.so; everything libhb itself provides (hb_buffer_*, hb_dict_*,
                           hb_log ...) is an undefined symbol of this library
@@ -20,7 +20,7 @@ REPO = ROOT.parent
 LIB = ROOT / "lib"
 
 NVCC_FLAGS = [
-    "-gencode", "arch=compute_100a,code=sm_100a",
+    "-gencode", "arch=compute_90a,code=sm_90a",
     "-O3", "-std=c++17", "-lineinfo",
     "-fmad=false",                  # the reference is built without FMA contraction (SURVEY.md 8a)
     "-Xcompiler", "-fPIC",
@@ -78,7 +78,7 @@ def build_cuda(force=False, verbose=False):
                 f.result()
     out = LIB / "libhbcu.so"
     if force or _newer(out, objs):
-        _run([nvcc_path(), "-shared", "-o", out] + objs + ["-gencode", "arch=compute_100a,code=sm_100a", "-cudart", "static", "-Xlinker", "--exclude-libs=ALL"], verbose)
+        _run([nvcc_path(), "-shared", "-o", out] + objs + ["-gencode", "arch=compute_90a,code=sm_90a", "-cudart", "static", "-Xlinker", "--exclude-libs=ALL"], verbose)
     return out
 
 

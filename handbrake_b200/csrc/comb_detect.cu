@@ -1,6 +1,6 @@
-// comb_detect.cu -- comb detection for sm_100a behind the C-ABI of include/hbcu.h.
+// comb_detect.cu -- comb detection for sm_90a behind the C-ABI of include/hbcu.h.
 //
-// Replaces (reference /root/reference/libhb):
+// Replaces (reference: HandBrake's libhb):
 //   detect_gamma_combed_segment / detect_combed_segment   templates/comb_detect_template.c:288-402, 789-933
 //   mask_filter_work / mask_erode_work / mask_dilate_work comb_detect.c:901-966, 726-792, 556-622
 //   check_filtered_combing_mask / check_combing_mask      comb_detect.c:221-276, 384-454
@@ -406,8 +406,7 @@ __device__ __forceinline__ int comb_rest(const CombParams &p, int pu2, int pu1, 
 // all kMaskRows rows from the column segment in registers; (2) every previous / next-frame sample some gated row of this lane
 // needs (rows y-1, y, y+1: consecutive output rows share two of three) issued back to back as predicated loads, then their
 // gamma lookups; (3) the motion tests and the metric, ballots and stores.  Round 1 let each gated row fetch its own six
-// samples inside the row loop: up to 16 exposed DRAM round trips per lane (8.3 long-scoreboard stalls per issue,
-// profiles/r02_comb_mask_ncu.json) and every sample fetched up to three times.
+// samples inside the row loop: up to 16 exposed DRAM round trips per lane and every sample fetched up to three times.
 template <typename PIX, bool GAMMA>
 __global__ void __launch_bounds__(256) comb_mask_bits2_kernel(const PIX *__restrict__ prev, const PIX *__restrict__ cur,
                                                              const PIX *__restrict__ next, uint32_t *__restrict__ bits,
@@ -856,7 +855,7 @@ int hbcu_comb_detect_run(hbcu_comb_detect_t *h, int64_t prev, int64_t cur, int64
             return -1;
         }
         dim3 mgrid((h->nwords + 7) / 8, (c.height + kMaskRows - 1) / kMaskRows);
-        // three-phase kernel by default (37.8 us against 49.2 us for the 4K 10-bit luma plane, profiles/r02_comb_mask2_ncu.json);
+        // three-phase kernel by default;
         // HBCU_COMB_MASK=1 selects the round-1 row-loop kernel (A/B, tests)
         static const int mask_impl = getenv("HBCU_COMB_MASK") ? atoi(getenv("HBCU_COMB_MASK")) : 2;
 #define MASK(K, PIX, A, B, D)                                                                                               \

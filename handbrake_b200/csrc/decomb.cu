@@ -1,7 +1,7 @@
-// decomb.cu -- decomb (yadif / cubic / blend line filters, bob, per-frame mode) for sm_100a
+// decomb.cu -- decomb (yadif / cubic / blend line filters, bob, per-frame mode) for sm_90a
 // behind the C-ABI of include/hbcu.h.
 //
-// Replaces (reference /root/reference/libhb):
+// Replaces (reference: HandBrake's libhb):
 //   cubic_interpolate_pixel/line  templates/decomb_template.c:43-107
 //   blend_filter_pixel/line       templates/decomb_template.c:279-361
 //   yadif_filter_line/YADIF_CHECK templates/decomb_template.c:482-710
@@ -279,7 +279,7 @@ __device__ __forceinline__ void yadif_px4(const FieldParams &fp, int x0, int y, 
 
 // one thread = 4 adjacent pixels of two consecutive output rows (one kept, one rebuilt): every warp carries the same
 // amount of work.  With one row per thread half of the warps (kept rows) retire at once and the SM runs at half its
-// already register-limited occupancy (ncu, profiles/r01h_decomb_ncu.txt: 12.9 % warps active, long-scoreboard bound).
+// already register-limited occupancy.
 template <typename PIX, bool CUBIC, bool EEDI>
 __device__ __forceinline__ void decomb_row4(const FieldParams &fp, int x0, int y)
 {

@@ -1,6 +1,6 @@
-// detelecine.cu -- the data-parallel half of pullup (inverse telecine) for sm_100a behind include/hbcu.h (SURVEY.md 8 f4).
+// detelecine.cu -- the data-parallel half of pullup (inverse telecine) for sm_90a behind include/hbcu.h (SURVEY.md 8 f4).
 //
-// Replaces, of reference /root/reference/libhb/detelecine.c:
+// Replaces, of the reference's libhb/detelecine.c:
 //   pullup_diff_y / pullup_licomb_y / pullup_var_y (:159-207) driven by pullup_compute_metric (:230-265)
 //   the max-reductions of pullup_compute_breaks (:369-374) and pullup_compute_affinity (:405-418)
 //   pullup_copy_field (:298-317) and the plane copies in and out of the pullup buffers (:1159-1164, :1250-1252)
@@ -215,9 +215,9 @@ int hbcu_detelecine_create(hbcu_detelecine_t **out, const hbcu_detelecine_config
     HBCU_CHECK(cudaSetDevice(cfg->device));
     cudaDeviceProp prop;
     HBCU_CHECK(cudaGetDeviceProperties(&prop, cfg->device));
-    if (prop.major < 10)
+    if (prop.major != 9 || prop.minor != 0)
     {
-        set_error("detelecine_create: device %d is sm_%d%d; this library is built for sm_100a only", cfg->device, prop.major, prop.minor);
+        set_error("detelecine_create: device %d is sm_%d%d; this library is built for sm_90a only", cfg->device, prop.major, prop.minor);
         return -1;
     }
     hbcu_detelecine_s *h = new (std::nothrow) hbcu_detelecine_s();
@@ -359,7 +359,7 @@ int hbcu_detelecine_metrics(hbcu_detelecine_t *h, int field, int picture, int pa
 static int reduction_grid(const hbcu_detelecine_s *h)
 {
     const int blocks = (h->metric_len + 255) / 256;
-    return blocks < 296 ? blocks : 296;                       // 2 CTAs per SM, grid-stride beyond that
+    return blocks < 264 ? blocks : 264;                       // 2 CTAs per SM of an H100 (132 SMs), grid-stride beyond that
 }
 
 int hbcu_detelecine_breaks(hbcu_detelecine_t *h, int field2, int field3, int slot)

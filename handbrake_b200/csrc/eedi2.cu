@@ -1,4 +1,4 @@
-// eedi2.cu -- EEDI2 edge-directed interpolation of one field to a full frame, for sm_100a.
+// eedi2.cu -- EEDI2 edge-directed interpolation of one field to a full frame, for sm_90a.
 //
 // Replaces the stage chain eedi2_interpolate_plane (reference libhb/templates/decomb_template.c:366-441)
 // and the stages it calls (libhb/templates/eedi2_template.c, HandBrake's fork of tritical's EEDI2):
@@ -194,8 +194,8 @@ template <int N> __device__ __forceinline__ uint32_t range_bits(int x0, int lo, 
 
 // The active samples of a stage cluster along edges: a vertical edge puts them into a few lanes of a warp, a horizontal
 // one into every lane of the few warps that own that row.  Handing every thread the samples of its own group serialises
-// the first case (measured: calc_directions 3.5x slower), pooling per warp serialises the second (a warp owning a fully
-// active 256-sample row segment needs 8 rounds while the rest of the GPU idles: 218 us vs 66 us, profiles/r01m).  So
+// the first case, pooling per warp serialises the second (a warp owning a fully active 256-sample row segment needs 8
+// rounds while the rest of the GPU idles).  So
 // the whole CTA (256 threads = 4 rows x 512 samples at 16 bit) pools its active samples in shared memory and deals them
 // out one per thread.  Every thread of the CTA must call this (no early returns before it).
 constexpr int kStageThreads = 256;             // stage kernels run blocks of 64 x 4 threads

@@ -1,6 +1,6 @@
-// hqdn3d.cu -- hqdn3d ("high quality 3-D denoise") for sm_100a behind the C-ABI of include/hbcu.h (SURVEY.md 8 f4).
+// hqdn3d.cu -- hqdn3d ("high quality 3-D denoise") for sm_90a behind the C-ABI of include/hbcu.h (SURVEY.md 8 f4).
 //
-// Replaces hqdn3d_denoise_spatial / _temporal / _depth (reference /root/reference/libhb/denoise.c:102-201).
+// Replaces hqdn3d_denoise_spatial / _temporal / _depth (reference libhb/denoise.c:102-201).
 // The reference sweeps a plane once, carrying three recursive low-passes: along the row (pixel_ant), down the column
 // (line_ant[]) and through time (frame_ant[]).  lowpass(prev, cur) = cur + coef[(prev - cur) >> (8 - LUT_BITS)] is a table
 // lookup, not a linear filter, so the recursions cannot be turned into scans -- but they separate:
@@ -582,9 +582,9 @@ int hbcu_hqdn3d_create(hbcu_hqdn3d_t **out, const hbcu_hqdn3d_config_t *cfg)
     HBCU_CHECK(cudaSetDevice(cfg->device));
     cudaDeviceProp prop;
     HBCU_CHECK(cudaGetDeviceProperties(&prop, cfg->device));
-    if (prop.major < 10)
+    if (prop.major != 9 || prop.minor != 0)
     {
-        set_error("hqdn3d_create: device %d is sm_%d%d; this library is built for sm_100a only", cfg->device, prop.major, prop.minor);
+        set_error("hqdn3d_create: device %d is sm_%d%d; this library is built for sm_90a only", cfg->device, prop.major, prop.minor);
         return -1;
     }
     hbcu_hqdn3d_s *h = new (std::nothrow) hbcu_hqdn3d_s();

@@ -1,4 +1,4 @@
-// lapsharp.cu -- Laplacian sharpen for sm_100a behind the C-ABI of include/hbcu.h.
+// lapsharp.cu -- Laplacian sharpen for sm_90a behind the C-ABI of include/hbcu.h.
 //
 // Replaces DEF_LAPSHARP_FUNC (reference libhb/lapsharp.c:125-182) and the frame batching of
 // mt_frame_filter.c:169-237: frames are independent, so each one is upload -> kernel -> download
@@ -46,8 +46,8 @@ struct LapFrame
     int max_value;
 };
 
-// int -> double without the conversion instruction: I2F.F64 issues at 15.7 lanes/clk/SM on B200, DADD at 63.8
-// (tools/latency_bench.cu).  0x43300000:lo is 2^52 + lo; subtracting the bias back is exact.
+// int -> double without the conversion instruction (a quarter-rate I2F.F64 against full-rate DADD on sm_90, CUDA C++
+// Programming Guide, arithmetic instruction throughput).  0x43300000:lo is 2^52 + lo; subtracting the bias back is exact.
 __device__ __forceinline__ double exact_i2d(int v)
 {
     return __dadd_rn(__hiloint2double(0x43300000, v ^ (int)0x80000000), -4503601774854144.0);      // -(2^52 + 2^31)
@@ -395,10 +395,8 @@ int launch_frame(hbcu_lapsharp_s *h, const void *const src[3], const int spitch_
     }
     const Geom &g0 = h->g[0];
     const bool vec = f.pl[0].vec && f.pl[1].vec && f.pl[2].vec;
-    // 4 rows per thread at 4 CTAs per SM (64 registers) measured best of {2, 4, 8 rows} x {2..6 CTAs}: 47.7k frames/s against
-    // 42.7k at 2 CTAs per SM (profiles/r02_lapsharp_variants.txt).  HBCU_LAP_VARIANT=8: the exact_i2d arithmetic instead of
-    // the conversion instructions -- measured SLOWER (43.9k against 46.8k on the same box: the two extra DADD and the xor cost
-    // more issue slots than the quarter-rate I2F.F64 costs pipe time), kept for the A/B only.
+    // 4 rows per thread at 4 CTAs per SM (64 registers).  HBCU_LAP_VARIANT=8: the exact_i2d arithmetic instead of the
+    // conversion instructions, kept for the A/B only.
     static const int variant = getenv("HBCU_LAP_VARIANT") ? atoi(getenv("HBCU_LAP_VARIANT")) : 0;
     constexpr int R = 4;
     dim3 blk(32, 8), grid(((g0.w + 3) / 4 + 31) / 32, (g0.h + 8 * R - 1) / (8 * R), 3);

@@ -1,6 +1,6 @@
-// nlmeans.cu -- NLMeans denoise for sm_100a behind the C-ABI of include/hbcu.h.
+// nlmeans.cu -- NLMeans denoise for sm_90a behind the C-ABI of include/hbcu.h.
 //
-// Replaces (reference /root/reference/libhb):
+// Replaces (reference: HandBrake's libhb):
 //   nlmeans_alloc / nlmeans_border      templates/nlmeans_template.c:20-101   -> pad_mirror_kernel
 //   build_integral_scalar / _sse2       templates/nlmeans_template.c:545-591, nlmeans_x86.c:20-149
 //   nlmeans_plane                       templates/nlmeans_template.c:593-717  -> nlmeans_tiled_kernel
@@ -46,10 +46,9 @@ constexpr int kMaxFrames = 32;    // NLMEANS_FRAMES_MAX
 constexpr int kMaxDevices = 64;   // per-device launch configuration flags (power of two)
 constexpr int kTileW     = 128;
 constexpr int kHalo      = 8;     // vertical halo of the shared-memory tiles (>= n/2 + r/2)
-// Horizontal halo.  Measured on B200 (tools/tma_test.cu): cp.async.bulk.tensor raises
-// "illegal instruction" unless the box's first byte in global memory is 16-byte aligned,
-// so the tile starts at bordered column X0 (a multiple of 128), i.e. the halo is the
-// whole 16-pixel mirror border.
+// Horizontal halo.  cp.async.bulk.tensor raises "illegal instruction" unless the box's
+// first byte in global memory is 16-byte aligned (tools/tma_test.cu), so the tile starts
+// at bordered column X0 (a multiple of 128), i.e. the halo is the whole 16-pixel mirror border.
 constexpr int kHaloX     = kBorder;
 constexpr int kTilePW    = kTileW + 2 * kHaloX;  // 160 elements per tile row
 constexpr int kThreads   = 256;
@@ -544,8 +543,7 @@ struct TiledParams
 };
 
 // The fast 8-bit kernel takes up to three planes in ONE launch (tiles of Y, U and V in one grid):
-// three separate launches end in three partial waves (510 + 135 + 135 CTAs on 148 SMs = 6 rounds),
-// one launch of all tiles needs 5.
+// three separate launches end in three partial waves, one launch of all tiles in one.
 struct FusedParams
 {
     int nplanes;
@@ -662,10 +660,10 @@ __global__ void __launch_bounds__(kThreads, 1) nlmeans_tiled_kernel(const __grid
 
 // ---------------------------------------------------------------------------
 // Fast 8-bit kernel (v2).  Same tiling and the same arithmetic results as the
-// kernel above, re-expressed for the B200 issue ports measured in
-// profiles/r01_microbench_instruction_throughput.txt:
+// kernel above, re-expressed for the SM's issue rates (CUDA C++ Programming Guide,
+// arithmetic instruction throughput, compute capability 9.0):
 //   * FADD/FMUL/FFMA issue at 4 warp-instr/clk/SM, integer ALU ops (PRMT, LOP3,
-//     IADD3, IMAD) at 2, F2I / I2F.U8 at 0.5, LDS at ~1.
+//     IADD3, IMAD) at 2, F2I / I2F.U8 at 0.5.
 //   * For 8-bit pixels every quantity of the patch distance is an integer
 //     below 2^24 (7*7*255^2 = 3.2M), so it is computed in fp32 EXACTLY: the
 //     squared difference is one FFMA into a running prefix sum, the patch-row
@@ -1489,7 +1487,7 @@ struct hbcu_nlmeans_s
     std::vector<CUtensorMap> maps;        // [slot*3+plane] TMA descriptors of the bordered planes
     std::vector<CUtensorMap> maps3;       // same planes, box height of the v3 8-bit kernel's tile
     std::vector<CUtensorMap> maps3_pre;   // the prefiltered planes (pre_mem), same box
-    int v3_nw, v3_rs, v3_tmem;            // v3 kernel shape (warps, rows per warp, accumulators in tensor memory); v3_nw == 0: off
+    int v3_nw, v3_rs;                     // v3 kernel shape (warps, rows per warp); v3_nw == 0: off
     float *d_exptable;                    // 3 x 128
     unsigned *d_range_flag;               // sticky: a 16-bit plane held a sample above kFast16Max (see nlmeans_fast16_kernel)
     cudaStream_t s_h2d, s_pad, s_compute, s_d2h;   // s_compute = s_comp[frame index & (n_comp - 1)] of the launch being queued
@@ -1622,10 +1620,10 @@ constexpr int kTH8 = 144;
 int g_ssd_variant = 1;     // 1: packed-byte VABSDIFF4 + IDP4A patch-row sums (measured 7 % faster), 0: fp32 prefix sums (FFMA);
                            // HBCU_NLMEANS_SSD selects (test/tuning hook: both are exact, tests run both)
 
-template <int NH, int NW, int RS, bool TMEM, int NBUF>
+template <int NH, int NW, int RS, int NBUF>
 int launch_v3(FusedParams &fp, cudaStream_t st)
 {
-    using L = V3Layout<NW, RS, TMEM, NBUF>;
+    using L = V3Layout<NW, RS, NBUF>;
     // function attributes live in the device's context: one flag per device (a second GPU would otherwise launch with
     // the default 48 KB limit -- 'invalid argument'; found by the first run of devices=0,1)
     static bool configured_on[kMaxDevices] = {};
@@ -1634,7 +1632,7 @@ int launch_v3(FusedParams &fp, cudaStream_t st)
     bool &configured = configured_on[dev_ & (kMaxDevices - 1)];
     if (!configured)
     {
-        HBCU_CHECK(cudaFuncSetAttribute(nlmeans_v3_kernel<NH, NW, RS, TMEM, NBUF>, cudaFuncAttributeMaxDynamicSharedMemorySize, L::kTotal));
+        HBCU_CHECK(cudaFuncSetAttribute(nlmeans_v3_kernel<NH, NW, RS, NBUF>, cudaFuncAttributeMaxDynamicSharedMemorySize, L::kTotal));
         configured = true;
     }
     int total = 0;
@@ -1645,15 +1643,15 @@ int launch_v3(FusedParams &fp, cudaStream_t st)
         total += fp.tiles_x[i] * ((fp.k[i].h + L::kTH - 1) / L::kTH);
     }
     fp.first_tile[fp.nplanes] = total;
-    nlmeans_v3_kernel<NH, NW, RS, TMEM, NBUF><<<total, NW * 32, L::kTotal, st>>>(fp);
+    nlmeans_v3_kernel<NH, NW, RS, NBUF><<<total, NW * 32, L::kTotal, st>>>(fp);
     hbcu::count_launch();
     return 0;
 }
 
-template <int NH, int NW, int RS, bool TMEM, int NBUF>
+template <int NH, int NW, int RS, int NBUF>
 int launch_v3w(FusedParams &fp, cudaStream_t st)
 {
-    using L = V3Layout<NW, RS, TMEM, NBUF, 2>;
+    using L = V3Layout<NW, RS, NBUF, 2>;
     // function attributes live in the device's context: one flag per device (a second GPU would otherwise launch with
     // the default 48 KB limit -- 'invalid argument'; found by the first run of devices=0,1)
     static bool configured_on[kMaxDevices] = {};
@@ -1662,7 +1660,7 @@ int launch_v3w(FusedParams &fp, cudaStream_t st)
     bool &configured = configured_on[dev_ & (kMaxDevices - 1)];
     if (!configured)
     {
-        HBCU_CHECK(cudaFuncSetAttribute(nlmeans_v3w_kernel<NH, NW, RS, TMEM, NBUF>, cudaFuncAttributeMaxDynamicSharedMemorySize, L::kTotal));
+        HBCU_CHECK(cudaFuncSetAttribute(nlmeans_v3w_kernel<NH, NW, RS, NBUF>, cudaFuncAttributeMaxDynamicSharedMemorySize, L::kTotal));
         configured = true;
     }
     int total = 0;
@@ -1673,17 +1671,17 @@ int launch_v3w(FusedParams &fp, cudaStream_t st)
         total += fp.tiles_x[i] * ((fp.k[i].h + L::kTH - 1) / L::kTH);
     }
     fp.first_tile[fp.nplanes] = total;
-    nlmeans_v3w_kernel<NH, NW, RS, TMEM, NBUF><<<total, NW * 32, L::kTotal, st>>>(fp);
+    nlmeans_v3w_kernel<NH, NW, RS, NBUF><<<total, NW * 32, L::kTotal, st>>>(fp);
     hbcu::count_launch();
     return 0;
 }
 
-// prefilter variant (patch distances from the pre-denoised planes): one plane per launch, 12 x 18, one compare buffer pair
+// prefilter variant (patch distances from the pre-denoised planes): one plane per launch, 12 x 10, one compare buffer pair
 template <int NH>
 int launch_v3_pre(FusedParams &fp, cudaStream_t st)
 {
-    constexpr int NW = 12, RS = 18;
-    using L = V3Layout<NW, RS, true, 1, 1, true>;
+    constexpr int NW = 12, RS = 10;
+    using L = V3Layout<NW, RS, 1, 1, true>;
     // function attributes live in the device's context: one flag per device (a second GPU would otherwise launch with
     // the default 48 KB limit -- 'invalid argument'; found by the first run of devices=0,1)
     static bool configured_on[kMaxDevices] = {};
@@ -1692,7 +1690,7 @@ int launch_v3_pre(FusedParams &fp, cudaStream_t st)
     bool &configured = configured_on[dev_ & (kMaxDevices - 1)];
     if (!configured)
     {
-        HBCU_CHECK(cudaFuncSetAttribute(nlmeans_v3_kernel<NH, NW, RS, true, 1, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, L::kTotal));
+        HBCU_CHECK(cudaFuncSetAttribute(nlmeans_v3_kernel<NH, NW, RS, 1, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, L::kTotal));
         configured = true;
     }
     int total = 0;
@@ -1703,15 +1701,16 @@ int launch_v3_pre(FusedParams &fp, cudaStream_t st)
         total += fp.tiles_x[i] * ((fp.k[i].h + L::kTH - 1) / L::kTH);
     }
     fp.first_tile[fp.nplanes] = total;
-    nlmeans_v3_kernel<NH, NW, RS, true, 1, true><<<total, NW * 32, L::kTotal, st>>>(fp);
+    nlmeans_v3_kernel<NH, NW, RS, 1, true><<<total, NW * 32, L::kTotal, st>>>(fp);
     hbcu::count_launch();
     return 0;
 }
 
-// v3 shapes built into the library: {warps, rows per warp, accumulators in tensor memory}.  Patch 9 (NH = 4) needs
-// 8 warps (its 9-row history does not fit 168 registers).
-struct V3Shape { int nw, rs, tmem; };
-constexpr V3Shape kV3Default = { 12, 18, 1 };      // measured on B200 (profiles/r02b_v3_shape_sweep.txt): 12x18 > 12x21 > 8x28 > 12x12 (shared-memory accumulators)
+// v3 shapes built into the library: {warps, rows per warp}.  Every variant has a 120-row tile (see V3Layout: the
+// shared-memory accumulators and tiles of the 16-bit and prefilter variants fill 221 KB of the 227 KB).  Patch 9
+// (NH = 4) needs 8 warps (its 9-row history does not fit 168 registers).
+struct V3Shape { int nw, rs; };
+constexpr V3Shape kV3Default = { 12, 10 };
 
 // rows of one TMA box of the v3 tile: V3Layout::kBoxRows restated for a run-time shape (the kernel's expect-tx byte
 // count and the tensor map must agree)
@@ -1721,34 +1720,29 @@ int v3_box_rows(int nw, int rs)
     return ((rows + loads - 1) / loads + 3) / 4 * 4;
 }
 
-bool v3_shape_ok(int nw, int rs, int tmem, int n_half)
+bool v3_shape_ok(int nw, int rs, int n_half)
 {
-    if (n_half == 4) return nw == 8 && rs == 27 && tmem == 1;
-    if (nw == 12 && rs == 18 && tmem == 1) return true;
-#ifdef HBCU_V3_SWEEP_SHAPES
-    if (nw == 12 && rs == 12 && tmem == 0) return true;
-    if (n_half == 3) return tmem == 1 && ((nw == 12 && rs == 21) || (nw == 8 && rs == 28));
-#endif
-    return false;
+    if (n_half == 4) return nw == 8 && rs == 15;
+    return nw == kV3Default.nw && rs == kV3Default.rs;
 }
 
 // the shape a plane with patch half-width n_half runs in, given the handle's shape (whose TMA box its tensor maps
-// were encoded for): patch 9 takes the 8-warp shape with the same tile height as 12 x 18
+// were encoded for): patch 9 takes the 8-warp shape with the same tile height as 12 x 10
 bool v3_pick(const hbcu_nlmeans_s *h, int n_half, V3Shape *out)
 {
     if (h->v3_nw <= 0) return false;
-    V3Shape s = { h->v3_nw, h->v3_rs, h->v3_tmem };
+    V3Shape s = { h->v3_nw, h->v3_rs };
     if (n_half == 4)
     {
-        s = V3Shape{ 8, 27, 1 };
+        s = V3Shape{ 8, 15 };
         if (v3_box_rows(s.nw, s.rs) != v3_box_rows(h->v3_nw, h->v3_rs) || s.nw * s.rs != h->v3_nw * h->v3_rs) return false;
     }
-    if (!v3_shape_ok(s.nw, s.rs, s.tmem, n_half)) return false;
+    if (!v3_shape_ok(s.nw, s.rs, n_half)) return false;
     *out = s;
     return true;
 }
 
-int launch_v3_nh(int nw, int rs, int tmem, FusedParams &fp, cudaStream_t st)
+int launch_v3_nh(int nw, int rs, FusedParams &fp, cudaStream_t st)
 {
     const int nh = fp.k[0].n_half;
     // every displacement row of this range must decompose into group shapes the kernels were built with
@@ -1759,21 +1753,15 @@ int launch_v3_nh(int nw, int rs, int tmem, FusedParams &fp, cudaStream_t st)
             if (!v3_group_known(ng, (12 + dx0) & 3, kOrgNone)) return 1;
             if (dx0 <= 0 && dx0 + ng > 0 && !v3_group_known(ng, (12 + dx0) & 3, -dx0)) return 1;
         }
-#define V3CASE(NH_, NW_, RS_, TM_, NB_) if (nh == NH_ && nw == NW_ && rs == RS_ && tmem == TM_) return launch_v3<NH_, NW_, RS_, TM_ != 0, NB_>(fp, st)
-    V3CASE(1, 12, 18, 1, 2); V3CASE(2, 12, 18, 1, 2); V3CASE(3, 12, 18, 1, 2);
-    V3CASE(4, 8, 27, 1, 2);
-#ifdef HBCU_V3_SWEEP_SHAPES
-    // the other shapes of profiles/r02b_v3_shape_sweep.txt (shared-memory accumulators, 252-row tile, 8 warps): built only
-    // with -DHBCU_V3_SWEEP_SHAPES, they cost minutes of compile time and lost the sweep
-    V3CASE(1, 12, 12, 0, 1); V3CASE(2, 12, 12, 0, 1); V3CASE(3, 12, 12, 0, 1);
-    V3CASE(3, 12, 21, 1, 2); V3CASE(3, 8, 28, 1, 2);
-#endif
+#define V3CASE(NH_, NW_, RS_, NB_) if (nh == NH_ && nw == NW_ && rs == RS_) return launch_v3<NH_, NW_, RS_, NB_>(fp, st)
+    V3CASE(1, 12, 10, 2); V3CASE(2, 12, 10, 2); V3CASE(3, 12, 10, 2);
+    V3CASE(4, 8, 15, 2);
 #undef V3CASE
     return 1;
 }
 
-// 16-bit planes: one shape (12 warps x 18 rows, accumulators in tensor memory, one compare buffer: two 74 KB tiles)
-constexpr V3Shape kV3wShape = { 12, 18, 1 };
+// 16-bit planes: one shape (12 warps x 10 rows, one compare buffer: two 42.5 KB tiles)
+constexpr V3Shape kV3wShape = { 12, 10 };
 
 int launch_v3w_nh(FusedParams &fp, cudaStream_t st)
 {
@@ -1786,9 +1774,9 @@ int launch_v3w_nh(FusedParams &fp, cudaStream_t st)
         }
     switch (fp.k[0].n_half)
     {
-        case 1: return launch_v3w<1, kV3wShape.nw, kV3wShape.rs, true, 1>(fp, st);
-        case 2: return launch_v3w<2, kV3wShape.nw, kV3wShape.rs, true, 1>(fp, st);
-        case 3: return launch_v3w<3, kV3wShape.nw, kV3wShape.rs, true, 1>(fp, st);
+        case 1: return launch_v3w<1, kV3wShape.nw, kV3wShape.rs, 1>(fp, st);
+        case 2: return launch_v3w<2, kV3wShape.nw, kV3wShape.rs, 1>(fp, st);
+        case 3: return launch_v3w<3, kV3wShape.nw, kV3wShape.rs, 1>(fp, st);
         default: return 1;
     }
 }
@@ -1851,7 +1839,7 @@ int launch_plane(hbcu_nlmeans_s *h, const KernelParams &kp, const int *slots, in
 {
     // prefilter modes on 8-bit planes: the v3 kernel's prefilter variant (VERDICT r1 missing 5: these settings used to fall
     // to the one-thread-per-pixel generic kernel); same validity conditions as the plain fast kernel
-    if (kp.use_pre && only_if_flag == nullptr && h->bps == 1 && h->impl == 0 && h->v3_nw == 12 && h->v3_rs == 18 && h->v3_tmem == 1 &&
+    if (kp.use_pre && only_if_flag == nullptr && h->bps == 1 && h->impl == 0 && h->v3_nw == kV3Default.nw && h->v3_rs == kV3Default.rs &&
         kp.n_half >= 1 && kp.n_half <= 3 && kp.n_half + kp.r_half <= kHalo && kp.nf <= kMaxTiledFrames && kp.wfact < 0.99f && kp.wfact > 1e-5f)
     {
         bool known = true;
@@ -1901,7 +1889,7 @@ int launch_plane(hbcu_nlmeans_s *h, const KernelParams &kp, const int *slots, in
             V3Shape vs;
             const bool v3 = v3_pick(h, kp.n_half, &vs);
             for (int f = 0; f < kp.nf; f++) fp.maps[0][f] = v3 ? h->maps3[slots[f] * 3 + plane] : tp.maps[f];
-            rc = v3 ? launch_v3_nh(vs.nw, vs.rs, vs.tmem, fp, h->s_compute) : launch_fast8_nh(fp, h->s_compute);
+            rc = v3 ? launch_v3_nh(vs.nw, vs.rs, fp, h->s_compute) : launch_fast8_nh(fp, h->s_compute);
         }
         else
             rc = h->bps == 1 ? launch_tiled_nh<uint8_t, kTH8>(tp, h->s_compute) : launch_tiled_nh<uint16_t, kTH16>(tp, h->s_compute);
@@ -2113,7 +2101,7 @@ int run_filter(hbcu_nlmeans_s *h, int64_t index, int navail, int oslot, void *co
             for (int f = 0; f < kps[pl].nf; f++) fp.maps[fp.nplanes][f] = (v3 ? h->maps3 : h->maps)[slots[pl][f] * 3 + pl];
             fp.nplanes++;
         }
-        if ((v3 ? launch_v3_nh(vs.nw, vs.rs, vs.tmem, fp, h->s_compute) : launch_fast8_nh(fp, h->s_compute)) != 0)
+        if ((v3 ? launch_v3_nh(vs.nw, vs.rs, fp, h->s_compute) : launch_fast8_nh(fp, h->s_compute)) != 0)
         { set_error("nlmeans: fused launch failed"); return -1; }
         HBCU_CHECK(cudaGetLastError());
         h->kernel_launches++;
@@ -2169,9 +2157,9 @@ int hbcu_nlmeans_create(hbcu_nlmeans_t **out, const hbcu_nlmeans_config_t *cfg)
     HBCU_CHECK(cudaSetDevice(cfg->device));
     cudaDeviceProp prop;
     HBCU_CHECK(cudaGetDeviceProperties(&prop, cfg->device));
-    if (prop.major < 10)
+    if (prop.major != 9 || prop.minor != 0)
     {
-        set_error("nlmeans_create: device %d is sm_%d%d; this library is built for sm_100a only", cfg->device, prop.major, prop.minor);
+        set_error("nlmeans_create: device %d is sm_%d%d; this library is built for sm_90a only", cfg->device, prop.major, prop.minor);
         return -1;
     }
     for (int pl = 0; pl < 3; pl++)
@@ -2203,19 +2191,19 @@ int hbcu_nlmeans_create(hbcu_nlmeans_t **out, const hbcu_nlmeans_config_t *cfg)
     h->impl = 0;
     if (const char *e = getenv("HBCU_NLMEANS_IMPL")) h->impl = atoi(e) >= 0 && atoi(e) <= 3 ? atoi(e) : 0;   // test hook
     if (const char *e = getenv("HBCU_NLMEANS_SSD")) g_ssd_variant = atoi(e);                                  // tuning hook
-    // v3 8-bit kernel shape; HBCU_NLMEANS_V3=off | "warps,rows,tmem" (tuning hook, see v3_shape_ok)
-    h->v3_nw = kV3Default.nw; h->v3_rs = kV3Default.rs; h->v3_tmem = kV3Default.tmem;
+    // v3 8-bit kernel shape; HBCU_NLMEANS_V3=off | "warps,rows" (tuning hook, see v3_shape_ok)
+    h->v3_nw = kV3Default.nw; h->v3_rs = kV3Default.rs;
     if (const char *e = getenv("HBCU_NLMEANS_V3"))
     {
-        int a = 0, b = 0, c = 0;
-        if (sscanf(e, "%d,%d,%d", &a, &b, &c) == 3 && v3_shape_ok(a, b, c, 3)) { h->v3_nw = a; h->v3_rs = b; h->v3_tmem = c; }
+        int a = 0, b = 0;
+        if (sscanf(e, "%d,%d", &a, &b) == 2 && v3_shape_ok(a, b, 3)) { h->v3_nw = a; h->v3_rs = b; }
         else h->v3_nw = 0;
     }
     if (h->bps != 1)
     {
         // 16-bit planes have one v3 shape (nlmeans_v3w_kernel); HBCU_NLMEANS_V3=off still selects the round-1 kernel
         const bool off = h->v3_nw == 0;
-        h->v3_nw = off ? 0 : kV3wShape.nw; h->v3_rs = kV3wShape.rs; h->v3_tmem = kV3wShape.tmem;
+        h->v3_nw = off ? 0 : kV3wShape.nw; h->v3_rs = kV3wShape.rs;
     }
     h->ring = cfg->ring_frames > 0 ? cfg->ring_frames : 8;
     h->out_slots = cfg->out_slots > 0 ? cfg->out_slots : 4;

@@ -2,9 +2,8 @@
 //
 // Same arithmetic contract as nlmeans_fast8_kernel (bit-identical to templates/nlmeans_template.c:593-717), same
 // tiling idea (TMA tile in shared memory, a lane marches down a 4-pixel-wide column strip keeping the vertical running
-// sum of horizontal patch-row sums and its N-row history in registers).  What changed, each item from the r01 ncu
-// capture (profiles/r01g_nlmeans_fused_ncu.json: 29 thread-instructions per pixel x displacement, 68 % issue,
-// ALU pipe 57 %, 35 % of the shared-memory wavefront budget):
+// sum of horizontal patch-row sums and its N-row history in registers).  What changed, each item aimed at the
+// instruction count per pixel and displacement:
 //   * group shape (NG displacements), byte offset of the compare window and the origin slot are template parameters:
 //     no per-row predicate/branch chains, and for the range-3 presets the three compare windows come straight out of
 //     the raw words with 6 funnel shifts per row instead of 13 (the source window is never re-aligned: only the
@@ -15,13 +14,12 @@
 //   * the three-row delay line of compare words is indexed by the unrolled row slot instead of being shifted: no MOVs;
 //   * warm-up rows are peeled: the steady-state loop has no "row >= NH" test;
 //   * the compare tile of frame 1 is in flight while frame 0 is compared with itself (second mbarrier);
-//   * accumulators (weight sum, pixel sum; 8 bytes per pixel) can live in TENSOR MEMORY (tcgen05.ld/st, 32x32b.x8:
-//     a lane's 4 x 2 floats are 8 columns of its own TMEM lane).  That takes their 16 wavefronts per row off the
-//     shared-memory pipe and -- shared memory no longer bounds the tile -- lets a warp march 18-20 rows instead of 12:
-//     the 2*NH warm-up rows drop from 50 % to 30-33 % of the patch-row-sum work.
+//   * accumulators (weight sum, pixel sum; 8 bytes per pixel) live in shared memory, a float4 per lane and array and row.
+//     Together with the tiles they bound the tile height: 120 rows (12 warps x 10) keep the largest variant (16-bit
+//     tiles, or the four tiles of the prefilter variant) inside the 227 KB an H100 block can have.
 #pragma once
 
-template <int NW, int RS, bool TMEM, int NBUF, int BPS = 1, bool PRE = false>
+template <int NW, int RS, int NBUF, int BPS = 1, bool PRE = false>
 struct V3Layout
 {
     static constexpr int kTH        = NW * RS;
@@ -30,7 +28,7 @@ struct V3Layout
     static constexpr int kRows      = kBoxRows * kLoads;                                 // >= kTH + 2 * kHalo; surplus rows are loaded, never used
     static constexpr int kRowBytes  = kTilePW * BPS;
     static constexpr int kTileBytes = kRows * kRowBytes;
-    static constexpr int kAccBytes  = TMEM ? 0 : kTH * kTileW * (int)sizeof(float);      // per accumulator array
+    static constexpr int kAccBytes  = kTH * kTileW * (int)sizeof(float);                 // per accumulator array
     static constexpr int kLutBytes  = kLutEntries * 32 * (int)sizeof(float);
     static constexpr int kOffCur    = 0;
     static constexpr int kOffCmp    = kOffCur + kTileBytes;
@@ -42,20 +40,17 @@ struct V3Layout
     static_assert(!PRE || NBUF == 1, "the prefilter variant keeps one compare buffer pair");
     static constexpr int kOffPs     = kOffWs + kAccBytes;
     static constexpr int kOffLut    = kOffPs + kAccBytes;
-    static constexpr int kOffBar    = kOffLut + kLutBytes;                               // 1 + NBUF mbarriers, TMEM base word
+    static constexpr int kOffBar    = kOffLut + kLutBytes;                               // 1 + NBUF mbarriers
     static constexpr int kUsed      = kOffBar + 64;
-    // one CTA per SM by construction (the TMEM variant allocates all 512 columns; a second resident CTA would spin)
+    // one CTA per SM by construction (every variant needs more than half of the SM's shared memory)
     static constexpr int kTotal     = kUsed < 117 * 1024 ? 117 * 1024 : kUsed;
     static_assert(kBoxRows <= 256, "TMA box rows");
     static_assert((kBoxRows * kRowBytes) % 128 == 0, "TMA destination must stay 128-byte aligned");
-    static_assert(!TMEM || ((NW + 3) / 4 * RS * 8 <= 512), "accumulators must fit 512 TMEM columns per lane quarter");
     static_assert(kTotal <= 227 * 1024, "shared memory");
 };
 
-// accumulator rows of one warp: shared memory (float4 per lane and array) or tensor memory (8 columns per lane)
-template <bool TMEM> struct V3Acc;
-
-template <> struct V3Acc<false>
+// accumulator rows of one warp in shared memory (float4 per lane and array)
+struct V3Acc
 {
     float *ws, *ps;     // this lane's first row
     __device__ __forceinline__ void load(int r, uint32_t (&v)[8]) const
@@ -73,62 +68,17 @@ template <> struct V3Acc<false>
     __device__ __forceinline__ void wait_store() const {}
 };
 
-template <> struct V3Acc<true>
+// fp32 pairs (pixels 0/2 and 1/3 of a lane's four): each half is one IEEE round-to-nearest (or toward-zero) fp32
+// operation.  The _rn/_rz intrinsics are never contracted into an FMA (the reference rounds the product before it adds).
+__device__ __forceinline__ float2 v3_pack2(float a, float b) { return make_float2(a, b); }
+__device__ __forceinline__ void v3_unpack2(float2 v, float &a, float &b)
 {
-    uint32_t taddr;     // lane quarter of this warp (bits 31..16) + first column of its strip
-    __device__ __forceinline__ void load(int r, uint32_t (&v)[8]) const
-    {
-        asm volatile("tcgen05.ld.sync.aligned.32x32b.x8.b32 {%0, %1, %2, %3, %4, %5, %6, %7}, [%8];"
-                     : "=r"(v[0]), "=r"(v[1]), "=r"(v[2]), "=r"(v[3]), "=r"(v[4]), "=r"(v[5]), "=r"(v[6]), "=r"(v[7])
-                     : "r"(taddr + (uint32_t)r * 8u));
-    }
-    // the registers are tied to the wait so that no consumer is scheduled above it
-    __device__ __forceinline__ void wait_load(uint32_t (&v)[8]) const
-    {
-        asm volatile("tcgen05.wait::ld.sync.aligned;"
-                     : "+r"(v[0]), "+r"(v[1]), "+r"(v[2]), "+r"(v[3]), "+r"(v[4]), "+r"(v[5]), "+r"(v[6]), "+r"(v[7]) :: "memory");
-    }
-    __device__ __forceinline__ void store(int r, const uint32_t (&v)[8]) const
-    {
-        asm volatile("tcgen05.st.sync.aligned.32x32b.x8.b32 [%0], {%1, %2, %3, %4, %5, %6, %7, %8};"
-                     :: "r"(taddr + (uint32_t)r * 8u), "r"(v[0]), "r"(v[1]), "r"(v[2]), "r"(v[3]), "r"(v[4]), "r"(v[5]), "r"(v[6]), "r"(v[7])
-                     : "memory");
-    }
-    __device__ __forceinline__ void wait_store() const { asm volatile("tcgen05.wait::st.sync.aligned;" ::: "memory"); }
-};
-
-// packed fp32 pairs (sm_100 add/mul.f32x2): each half is an IEEE round-to-nearest (or toward-zero) fp32 operation
-__device__ __forceinline__ uint64_t v3_pack2(float a, float b)
-{
-    uint64_t r;
-    asm("mov.b64 %0, {%1, %2};" : "=l"(r) : "f"(a), "f"(b));
-    return r;
+    a = v.x;
+    b = v.y;
 }
-__device__ __forceinline__ void v3_unpack2(uint64_t v, float &a, float &b)
-{
-    asm("mov.b64 {%0, %1}, %2;" : "=f"(a), "=f"(b) : "l"(v));
-}
-__device__ __forceinline__ uint64_t v3_add2(uint64_t a, uint64_t b)
-{
-    uint64_t r;
-    asm("add.rn.f32x2 %0, %1, %2;" : "=l"(r) : "l"(a), "l"(b));
-    return r;
-}
-__device__ __forceinline__ uint64_t v3_add2_rz(uint64_t a, uint64_t b)
-{
-    uint64_t r;
-    asm("add.rz.f32x2 %0, %1, %2;" : "=l"(r) : "l"(a), "l"(b));
-    return r;
-}
-// product of two pairs of NON-NEGATIVE floats.  Written as fma(a, b, +0): ptxas contracts mul.rn.f32x2 + add.rn.f32x2
-// into one FFMA2 even under -fmad=false (seen in the SASS; the reference rounds the product before it adds), and it
-// cannot fold an explicit fma.  a * b + (+0) == rn(a * b) whenever the product is not -0, which weights and pixels never are.
-__device__ __forceinline__ uint64_t v3_mul2(uint64_t a, uint64_t b)
-{
-    uint64_t r;
-    asm("fma.rn.f32x2 %0, %1, %2, %3;" : "=l"(r) : "l"(a), "l"(b), "l"(0ull));
-    return r;
-}
+__device__ __forceinline__ float2 v3_add2(float2 a, float2 b) { return make_float2(__fadd_rn(a.x, b.x), __fadd_rn(a.y, b.y)); }
+__device__ __forceinline__ float2 v3_add2_rz(float2 a, float2 b) { return make_float2(__fadd_rz(a.x, b.x), __fadd_rz(a.y, b.y)); }
+__device__ __forceinline__ float2 v3_mul2(float2 a, float2 b) { return make_float2(__fmul_rn(a.x, b.x), __fmul_rn(a.y, b.y)); }
 // position of pixel i of a lane's four in the accumulator words (pairs (0, 2) and (1, 3))
 __device__ __forceinline__ constexpr int v3_acc_slot(int i) { return (i & 1) * 2 + (i >> 1); }
 
@@ -302,16 +252,15 @@ struct V3Group
                 p0 = P[KP][0];
                 p1 = P[KP][1];
             }
-            // pixels 0/2 and 1/3 of the lane's four travel as packed pairs (add/mul.rn.f32x2: two IEEE fp32 operations per
-            // issue slot, same rounding as the scalar instructions); accumulator words are stored in that order:
+            // pixels 0/2 and 1/3 of the lane's four travel as pairs; accumulator words are stored in that order:
             // {ws0, ws2, ws1, ws3, ps0, ps2, ps1, ps3}
-            uint64_t pix2[NG + 1];                        // (compare pixel j, compare pixel j + 2) as floats
+            float2 pix2[NG + 1];                          // (compare pixel j, compare pixel j + 2) as floats
 #pragma unroll
             for (int j = 0; j < NG + 1; j++)
                 pix2[j] = v3_add2(v3_pack2(byte_as_biased_float(j < 4 ? p0 : p1, j & 3), byte_as_biased_float(j + 2 < 4 ? p0 : p1, (j + 2) & 3)),
                                   v3_pack2(-8388608.0f, -8388608.0f));
             acc.wait_load(accv);                          // issued at the top of the step: the patch-row sums covered its latency
-            uint64_t W[NG][2];                            // weights of pixels (0, 2) and (1, 3)
+            float2 W[NG][2];                              // weights of pixels (0, 2) and (1, 3)
 #pragma unroll
             for (int g = 0; g < NG; g++)
             {
@@ -330,7 +279,7 @@ struct V3Group
                     W[g][h] = v3_pack2(w0, w1);
                 }
             }
-            uint64_t ws2[2], ps2[2];
+            float2 ws2[2], ps2[2];
 #pragma unroll
             for (int h = 0; h < 2; h++)
             {
@@ -446,11 +395,11 @@ __host__ __device__ inline bool v3_group_known(int ng, int ob, int org)
     return false;
 }
 
-template <int NH, int NW, int RS, bool TMEM, int NBUF, bool PRE = false>
+template <int NH, int NW, int RS, int NBUF, bool PRE = false>
 __global__ void __launch_bounds__(NW * 32, 1) nlmeans_v3_kernel(const __grid_constant__ FusedParams fp)
 {
     constexpr int kThreads = NW * 32;
-    using L = V3Layout<NW, RS, TMEM, NBUF, 1, PRE>;
+    using L = V3Layout<NW, RS, NBUF, 1, PRE>;
     int pl = 0;
     while (pl + 1 < fp.nplanes && (int)blockIdx.x >= fp.first_tile[pl + 1]) pl++;
     const KernelParams &p = fp.k[pl];
@@ -461,7 +410,6 @@ __global__ void __launch_bounds__(NW * 32, 1) nlmeans_v3_kernel(const __grid_con
     uint8_t *cur  = smem + L::kOffCur;
     float *lut    = reinterpret_cast<float *>(smem + L::kOffLut);
     uint64_t *bar = reinterpret_cast<uint64_t *>(smem + L::kOffBar);           // [0] current tile, [1 + b] compare buffer b
-    uint32_t *tmem_base_slot = reinterpret_cast<uint32_t *>(smem + L::kOffBar + 8 * (1 + NBUF));
 
     const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
     const int X0 = (tile % fp.tiles_x[pl]) * kTileW, Y0 = (tile / fp.tiles_x[pl]) * L::kTH;
@@ -472,15 +420,7 @@ __global__ void __launch_bounds__(NW * 32, 1) nlmeans_v3_kernel(const __grid_con
         for (int b = 0; b < 1 + NBUF; b++) mbar_init(bar + b, 1);
         asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
     }
-    __syncwarp();
-    if (TMEM && warp == 0)
-    {
-        asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], 512;" :: "r"(smem_u32(tmem_base_slot)) : "memory");
-        asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-    }
-    if (TMEM) asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
     __syncthreads();
-    if (TMEM) asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
     if (tid == 0)
     {
         mbar_expect_tx(bar, L::kTileBytes * (PRE ? 2 : 1));
@@ -507,27 +447,16 @@ __global__ void __launch_bounds__(NW * 32, 1) nlmeans_v3_kernel(const __grid_con
     const int seg_y0 = warp * RS;
     int rows = p.h - (Y0 + seg_y0);                                     // rows of this warp's strip inside the plane
     rows = rows < 0 ? 0 : (rows > RS ? RS : rows);
-    V3Acc<TMEM> acc;
-    if constexpr (TMEM)
+    V3Acc acc;
+    float *acc_ws = reinterpret_cast<float *>(smem + L::kOffWs);
+    float *acc_ps = reinterpret_cast<float *>(smem + L::kOffPs);
+    for (int i = tid; i < L::kTH * kTileW; i += kThreads)
     {
-        const uint32_t base = *tmem_base_slot;
-        acc.taddr = base + ((uint32_t)(warp & 3) << 21) + (uint32_t)((warp >> 2) * RS * 8);   // lane 32 * (warp % 4) in bits 31..16
-        uint32_t z[8] = { 0, 0, 0, 0, 0, 0, 0, 0 };
-        for (int r = 0; r < RS; r++) acc.store(r, z);
-        acc.wait_store();
+        acc_ws[i] = 0.f;
+        acc_ps[i] = 0.f;
     }
-    else
-    {
-        float *acc_ws = reinterpret_cast<float *>(smem + L::kOffWs);
-        float *acc_ps = reinterpret_cast<float *>(smem + L::kOffPs);
-        for (int i = tid; i < L::kTH * kTileW; i += kThreads)
-        {
-            acc_ws[i] = 0.f;
-            acc_ps[i] = 0.f;
-        }
-        acc.ws = acc_ws + seg_y0 * kTileW + lane * 4;
-        acc.ps = acc_ps + seg_y0 * kTileW + lane * 4;
-    }
+    acc.ws = acc_ws + seg_y0 * kTileW + lane * 4;
+    acc.ps = acc_ps + seg_y0 * kTileW + lane * 4;
     mbar_wait(bar, 0);
     __syncthreads();
 
@@ -613,16 +542,6 @@ __global__ void __launch_bounds__(NW * 32, 1) nlmeans_v3_kernel(const __grid_con
                 if (X0 + x + i < p.w) drow[i] = o[i];
         }
     }
-    if (TMEM)
-    {
-        asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-        __syncthreads();
-        if (warp == 0)
-        {
-            asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-            asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, 512;" :: "r"(*tmem_base_slot) : "memory");
-        }
-    }
 }
 
 
@@ -634,8 +553,7 @@ __global__ void __launch_bounds__(NW * 32, 1) nlmeans_v3_kernel(const __grid_con
 // of horizontal patch-row sums in registers.  The squared differences have no packed-integer instruction at this width;
 // they are fp32 integers instead -- every value stays below 2^24, so every add/fma is exact in ANY order, which frees the
 // grouping: the four windows of a row share their middle (27 fp32 operations per displacement and row instead of a
-// 10-long prefix chain plus window differences; packing two displacements into f32x2 pairs was costed and dropped -- the
-// operand pairs cost as many PRMTs as the packed arithmetic saves).  V is a plain integer here
+// 10-long prefix chain plus window differences).  V is a plain integer here
 // (49 x 1023^2 does not fit the 2^23-biased-float trick of the 8-bit kernel): I2FP + FMUL.SAT.
 // The compare pixels of the output row are re-read from shared memory (no 7-row delay line of words in registers).
 template <int NH, int NG, int OB, int ORG, class ACC>
@@ -738,14 +656,14 @@ struct V3Group16
             uint32_t wp[NWP];
 #pragma unroll
             for (int j = 0; j < NWP; j++) wp[j] = prow[r * PW + j];
-            uint64_t pix2[NG + 1];                        // (compare pixel j, compare pixel j + 2) as floats
+            float2 pix2[NG + 1];                          // (compare pixel j, compare pixel j + 2) as floats
 #pragma unroll
             for (int j = 0; j < NG + 1; j++)
                 pix2[j] = v3_add2(v3_pack2(half_as_biased_float(wp[(OP + j) >> 1], (OP + j) & 1),
                                            half_as_biased_float(wp[(OP + j + 2) >> 1], (OP + j + 2) & 1)),
                                   v3_pack2(-kBias, -kBias));
             acc.wait_load(accv);
-            uint64_t W[NG][2];
+            float2 W[NG][2];
 #pragma unroll
             for (int g = 0; g < NG; g++)
             {
@@ -764,7 +682,7 @@ struct V3Group16
                     W[g][h] = v3_pack2(w0, w1);
                 }
             }
-            uint64_t ws2[2], ps2[2];
+            float2 ws2[2], ps2[2];
 #pragma unroll
             for (int h = 0; h < 2; h++)
             {
@@ -837,12 +755,12 @@ __device__ __forceinline__ void v3_group16(const uint32_t *__restrict__ cur, con
     g.run(rows);
 }
 
-template <int NH, int NW, int RS, bool TMEM, int NBUF>
+template <int NH, int NW, int RS, int NBUF>
 __global__ void __launch_bounds__(NW * 32, 1) nlmeans_v3w_kernel(const __grid_constant__ FusedParams fp)
 {
     if (*fp.range_flag != 0u) return;               // samples above 10 bit seen: the integer kernel takes over
     constexpr int kThreads = NW * 32;
-    using L = V3Layout<NW, RS, TMEM, NBUF, 2>;
+    using L = V3Layout<NW, RS, NBUF, 2>;
     int pl = 0;
     while (pl + 1 < fp.nplanes && (int)blockIdx.x >= fp.first_tile[pl + 1]) pl++;
     const KernelParams &p = fp.k[pl];
@@ -852,7 +770,6 @@ __global__ void __launch_bounds__(NW * 32, 1) nlmeans_v3w_kernel(const __grid_co
     uint8_t *cur  = smem + L::kOffCur;
     float *lut    = reinterpret_cast<float *>(smem + L::kOffLut);
     uint64_t *bar = reinterpret_cast<uint64_t *>(smem + L::kOffBar);
-    uint32_t *tmem_base_slot = reinterpret_cast<uint32_t *>(smem + L::kOffBar + 8 * (1 + NBUF));
 
     const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
     const int X0 = (tile % fp.tiles_x[pl]) * kTileW, Y0 = (tile / fp.tiles_x[pl]) * L::kTH;
@@ -863,15 +780,7 @@ __global__ void __launch_bounds__(NW * 32, 1) nlmeans_v3w_kernel(const __grid_co
         for (int b = 0; b < 1 + NBUF; b++) mbar_init(bar + b, 1);
         asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
     }
-    __syncwarp();
-    if (TMEM && warp == 0)
-    {
-        asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], 512;" :: "r"(smem_u32(tmem_base_slot)) : "memory");
-        asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-    }
-    if (TMEM) asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
     __syncthreads();
-    if (TMEM) asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
     if (tid == 0)
     {
         mbar_expect_tx(bar, L::kTileBytes);
@@ -892,27 +801,16 @@ __global__ void __launch_bounds__(NW * 32, 1) nlmeans_v3w_kernel(const __grid_co
     const int seg_y0 = warp * RS;
     int rows = p.h - (Y0 + seg_y0);
     rows = rows < 0 ? 0 : (rows > RS ? RS : rows);
-    V3Acc<TMEM> acc;
-    if constexpr (TMEM)
+    V3Acc acc;
+    float *acc_ws = reinterpret_cast<float *>(smem + L::kOffWs);
+    float *acc_ps = reinterpret_cast<float *>(smem + L::kOffPs);
+    for (int i = tid; i < L::kTH * kTileW; i += kThreads)
     {
-        const uint32_t base = *tmem_base_slot;
-        acc.taddr = base + ((uint32_t)(warp & 3) << 21) + (uint32_t)((warp >> 2) * RS * 8);
-        uint32_t z[8] = { 0, 0, 0, 0, 0, 0, 0, 0 };
-        for (int r = 0; r < RS; r++) acc.store(r, z);
-        acc.wait_store();
+        acc_ws[i] = 0.f;
+        acc_ps[i] = 0.f;
     }
-    else
-    {
-        float *acc_ws = reinterpret_cast<float *>(smem + L::kOffWs);
-        float *acc_ps = reinterpret_cast<float *>(smem + L::kOffPs);
-        for (int i = tid; i < L::kTH * kTileW; i += kThreads)
-        {
-            acc_ws[i] = 0.f;
-            acc_ps[i] = 0.f;
-        }
-        acc.ws = acc_ws + seg_y0 * kTileW + lane * 4;
-        acc.ps = acc_ps + seg_y0 * kTileW + lane * 4;
-    }
+    acc.ws = acc_ws + seg_y0 * kTileW + lane * 4;
+    acc.ps = acc_ps + seg_y0 * kTileW + lane * 4;
     mbar_wait(bar, 0);
     __syncthreads();
 
@@ -983,16 +881,6 @@ __global__ void __launch_bounds__(NW * 32, 1) nlmeans_v3w_kernel(const __grid_co
 #pragma unroll
             for (int i = 0; i < 4; i++)
                 if (X0 + x + i < p.w) drow[i] = o[i];
-        }
-    }
-    if (TMEM)
-    {
-        asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-        __syncthreads();
-        if (warp == 0)
-        {
-            asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-            asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, 512;" :: "r"(*tmem_base_slot) : "memory");
         }
     }
 }

@@ -1,6 +1,6 @@
-// unsharp.cu -- unsharp mask and chroma smoothing for sm_100a behind the C-ABI of include/hbcu.h.
+// unsharp.cu -- unsharp mask and chroma smoothing for sm_90a behind the C-ABI of include/hbcu.h.
 //
-// Replaces (reference /root/reference/libhb): DEF_UNSHARP_FUNC (unsharp.c:88-168) and DEF_CHROMA_SMOOTH_FUNC
+// Replaces (reference: HandBrake's libhb): DEF_UNSHARP_FUNC (unsharp.c:88-168) and DEF_CHROMA_SMOOTH_FUNC
 // (chroma_smooth.c:86-168) -- with lapsharp the three clients of hb_filter_mt_frame (common.c:5497-5517); the frame
 // batching of mt_frame_filter.c:169-237 becomes frames in flight on streams, as in lapsharp.cu.
 //
@@ -297,9 +297,9 @@ int hbcu_unsharp_create(hbcu_unsharp_t **out, const hbcu_unsharp_config_t *cfg)
     HBCU_CHECK(cudaSetDevice(cfg->device));
     cudaDeviceProp prop;
     HBCU_CHECK(cudaGetDeviceProperties(&prop, cfg->device));
-    if (prop.major < 10)
+    if (prop.major != 9 || prop.minor != 0)
     {
-        set_error("unsharp_create: device %d is sm_%d%d; this library is built for sm_100a only", cfg->device, prop.major, prop.minor);
+        set_error("unsharp_create: device %d is sm_%d%d; this library is built for sm_90a only", cfg->device, prop.major, prop.minor);
         return -1;
     }
     hbcu_unsharp_s *h = new (std::nothrow) hbcu_unsharp_s();

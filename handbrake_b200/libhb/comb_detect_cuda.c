@@ -1,5 +1,5 @@
 /* comb_detect_cuda.c -- hb_filter_comb_detect_cuda: drop-in for hb_filter_comb_detect
- * (reference libhb/comb_detect.c:129-140) running on a B200 through include/hbcu.h.
+ * (reference libhb/comb_detect.c:129-140) running on an H100 through include/hbcu.h.
  *
  * Same plugin surface as the reference: same settings keys and defaults
  * (comb_detect.c:1118-1140), thresholds scaled by depth (:1152-1153), gamma table
@@ -65,7 +65,7 @@ hb_filter_object_t hb_filter_comb_detect_cuda =
 {
     .id                = HB_FILTER_COMB_DETECT,
     .enforce_order     = 1,
-    .name              = "Comb Detect (CUDA sm_100a)",
+    .name              = "Comb Detect (CUDA sm_90a)",
     .short_name        = "comb-detect",
     .settings          = NULL,
     .init              = comb_detect_cuda_init,

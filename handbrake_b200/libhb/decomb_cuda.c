@@ -1,5 +1,5 @@
 /* decomb_cuda.c -- hb_filter_decomb_cuda: drop-in for hb_filter_decomb
- * (reference libhb/decomb.c:182-193) running on a B200 through include/hbcu.h.
+ * (reference libhb/decomb.c:182-193) running on an H100 through include/hbcu.h.
  *
  * Same plugin surface as the reference: settings keys and defaults (decomb.c:234-273),
  * prev/cur/next window with the first frame as its own predecessor and the last as its
@@ -73,7 +73,7 @@ hb_filter_object_t hb_filter_decomb_cuda =
 {
     .id                = HB_FILTER_DECOMB,
     .enforce_order     = 1,
-    .name              = "Decomb (CUDA sm_100a)",
+    .name              = "Decomb (CUDA sm_90a)",
     .short_name        = "decomb",
     .settings          = NULL,
     .init              = decomb_cuda_init,

@@ -1,5 +1,5 @@
 /* denoise_cuda.c -- hb_filter_denoise_cuda: drop-in for hb_filter_denoise (hqdn3d, reference libhb/denoise.c:64-76,
- * 214-371) running on a B200 through include/hbcu.h (SURVEY.md 8 f4).
+ * 214-371) running on an H100 through include/hbcu.h (SURVEY.md 8 f4).
  *
  * Same settings keys and default chain (denoise.c:237-266).  The coefficient tables are the numeric contract
  * (hqdn3d_precalc_coef, denoise.c:78-94): they are computed here, on the host, with the expressions of the reference and
@@ -46,7 +46,7 @@ hb_filter_object_t hb_filter_denoise_cuda =
 {
     .id                = HB_FILTER_DENOISE,
     .enforce_order     = 1,
-    .name              = "Denoise (hqdn3d, CUDA sm_100a)",
+    .name              = "Denoise (hqdn3d, CUDA sm_90a)",
     .short_name        = "hqdn3d",
     .settings          = NULL,
     .init              = denoise_cuda_init,

@@ -1,5 +1,5 @@
 /* detelecine_cuda.c -- hb_filter_detelecine_cuda: drop-in for hb_filter_detelecine (pullup inverse telecine, reference
- * libhb/detelecine.c:113-133, 1006-1277) running on a B200 through include/hbcu.h (SURVEY.md 8 f4).
+ * libhb/detelecine.c:113-133, 1006-1277) running on an H100 through include/hbcu.h (SURVEY.md 8 f4).
  *
  * Division of labour.  pullup is a small state machine over a queue of fields -- which field is compared with which,
  * where the cadence breaks, how many fields make the next frame and which of them -- fed by three per-block metrics of
@@ -70,7 +70,7 @@ hb_filter_object_t hb_filter_detelecine_cuda =
 {
     .id                = HB_FILTER_DETELECINE,
     .enforce_order     = 1,
-    .name              = "Detelecine (pullup, CUDA sm_100a)",
+    .name              = "Detelecine (pullup, CUDA sm_90a)",
     .short_name        = "detelecine",
     .settings          = NULL,
     .init              = detelecine_cuda_init,

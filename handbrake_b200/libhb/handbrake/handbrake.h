@@ -11,7 +11,7 @@
  * to compile the reference's own filter sources unmodified (they
  * `#include "handbrake/handbrake.h"`, which resolves here first).
  *
- * Mirrors (reference @ /root/reference/libhb):
+ * Mirrors (reference: HandBrake's libhb):
  *   hb_buffer_t, hb_buffer_settings_s, hb_image_format_s  handbrake/internal.h:63-165
  *   hb_image_stride/width/height                          handbrake/internal.h:220-254
  *   hb_filter_object_t, hb_filter_init_t, HB_FILTER_*     handbrake/common.h:1628-1711
@@ -170,7 +170,7 @@ struct hb_image_format_s
     int window_width, window_height;
 };
 
-/* storage_type gains the B200 backings the north-star asks for:
+/* storage_type gains the device backings:
  * HBCU_PINNED  : data lives in cudaHostAlloc'ed (page-locked) host memory
  * HBCU_DEVICE  : plane[].data are device pointers; storage = owning context */
 struct hb_buffer_s

@@ -1,6 +1,6 @@
 /* lapsharp_cuda.c -- hb_filter_lapsharp_cuda: drop-in for hb_filter_lapsharp wrapped in
  * hb_filter_mt_frame (reference libhb/lapsharp.c:112-123, mt_frame_filter.c:45-237,
- * common.c:5497-5517) running on a B200 through include/hbcu.h.
+ * common.c:5497-5517) running on an H100 through include/hbcu.h.
  *
  * Same settings (y-/cb-/cr-strength, -kernel with the names lap/isolap/log/isolog), same
  * cascade/defaults/sanitising (lapsharp.c:228-297).  mt_frame's "collect cpu_count frames,
@@ -48,7 +48,7 @@ hb_filter_object_t hb_filter_lapsharp_cuda =
 {
     .id                = HB_FILTER_LAPSHARP,
     .enforce_order     = 1,
-    .name              = "Sharpen (lapsharp, CUDA sm_100a)",
+    .name              = "Sharpen (lapsharp, CUDA sm_90a)",
     .short_name        = "lapsharp",
     .settings          = NULL,
     .init              = lapsharp_cuda_init,

@@ -1,5 +1,5 @@
 /* nlmeans_cuda.c -- hb_filter_nlmeans_cuda: drop-in for hb_filter_nlmeans
- * (reference libhb/nlmeans.c:202-213) whose per-pixel work runs on a B200
+ * (reference libhb/nlmeans.c:202-213) whose per-pixel work runs on an H100
  * through the C-ABI in include/hbcu.h.  Host side stays C, as in libhb.
  *
  * Same plugin surface as the reference: same settings_template and keys, same
@@ -137,7 +137,7 @@ hb_filter_object_t hb_filter_nlmeans_cuda =
 {
     .id                = HB_FILTER_NLMEANS,
     .enforce_order     = 1,
-    .name              = "Denoise (nlmeans, CUDA sm_100a)",
+    .name              = "Denoise (nlmeans, CUDA sm_90a)",
     .short_name        = "nlmeans",
     .settings          = NULL,
     .init              = nlmeans_cuda_init,

@@ -1,6 +1,6 @@
 /* unsharp_cuda.c -- hb_filter_unsharp_cuda and hb_filter_chroma_smooth_cuda: drop-ins for hb_filter_unsharp /
  * hb_filter_chroma_smooth wrapped in hb_filter_mt_frame (reference libhb/unsharp.c:70-84, chroma_smooth.c:72-86,
- * mt_frame_filter.c:45-237, common.c:5497-5517) running on a B200 through include/hbcu.h (SURVEY.md 8 f2).
+ * mt_frame_filter.c:45-237, common.c:5497-5517) running on an H100 through include/hbcu.h (SURVEY.md 8 f2).
  *
  * Same settings keys, cascade, defaults and sanitising (unsharp.c:213-276, chroma_smooth.c:196-270).  mt_frame's
  * "collect cpu_count frames, run them on cpu_count threads, emit them together" becomes frames in flight on the
@@ -51,7 +51,7 @@ hb_filter_object_t hb_filter_unsharp_cuda =
 {
     .id                = HB_FILTER_UNSHARP,
     .enforce_order     = 1,
-    .name              = "Sharpen (unsharp, CUDA sm_100a)",
+    .name              = "Sharpen (unsharp, CUDA sm_90a)",
     .short_name        = "unsharp",
     .settings          = NULL,
     .init              = unsharp_cuda_init,
@@ -64,7 +64,7 @@ hb_filter_object_t hb_filter_chroma_smooth_cuda =
 {
     .id                = HB_FILTER_CHROMA_SMOOTH,
     .enforce_order     = 1,
-    .name              = "Chroma Smooth (CUDA sm_100a)",
+    .name              = "Chroma Smooth (CUDA sm_90a)",
     .short_name        = "chromasmooth",
     .settings          = NULL,
     .init              = unsharp_cuda_init,

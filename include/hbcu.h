@@ -1,10 +1,10 @@
-/* hbcu.h -- C-ABI of the B200 (sm_100a) implementation of libhb's per-pixel
+/* hbcu.h -- C-ABI of the H100 (sm_90a) implementation of libhb's per-pixel
  * video-filter hot path.  Plain pointers and sizes only; no CUDA or torch types.
  *
  * This is the boundary a libhb maintainer binds: the filter objects in
  * handbrake_b200/libhb/ (nlmeans_cuda.c, ...) (drop-ins for hb_filter_nlmeans, ...) are
  * ordinary C that call ONLY the functions below.  Each group names the
- * reference code it replaces (paths relative to /root/reference/libhb).
+ * reference code it replaces (paths relative to HandBrake's libhb).
  *
  * Conventions
  *   - every function returns 0 on success, non-zero on failure;
@@ -16,7 +16,7 @@
  *     work.c:2527); different handles may be used from different threads concurrently.  All device work is queued
  *     on the handle's own non-blocking streams and ordered by events; calls return before the work has run unless
  *     they are named wait / sync / result.
- *   - nothing here falls back to the CPU: with no usable sm_100 device the
+ *   - nothing here falls back to the CPU: with no usable sm_90 device the
  *     create functions fail (=> filter init() returns non-zero, and libhb drops
  *     the filter exactly as for any failing init, work.c:1861-1868).
  */
@@ -190,7 +190,7 @@ int  hbcu_nlmeans_filter_frame(hbcu_nlmeans_t *h, int64_t index, int navail, hbc
 /* orders a caller-owned CUDA stream (passed as void*) after all work queued on the handle so far */
 int  hbcu_nlmeans_stream_wait(hbcu_nlmeans_t *h, void *cuda_stream);
 int  hbcu_nlmeans_sync(hbcu_nlmeans_t *h);
-/* implementation selector for tests: 0 = auto (tiled sm_100a kernel when the
+/* implementation selector for tests: 0 = auto (tiled sm_90a kernel when the
  * parameters fit, generic otherwise), 1 = force generic, 2 = force tiled,
  * 3 = tiled but integer-arithmetic variant (the one 16-bit planes use) */
 int  hbcu_nlmeans_set_impl(hbcu_nlmeans_t *h, int impl);

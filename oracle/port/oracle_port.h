@@ -1,7 +1,7 @@
 /* oracle_port.h -- TEST INFRASTRUCTURE, NOT PRODUCT CODE.
  *
  * Plain-C restatement of the reference's per-pixel algorithms for the hot path
- * (HandBrake libhb, /root/reference/libhb), written independently of the
+ * (HandBrake libhb), written independently of the
  * reference's data flow (no integral images, no bordered copies) so that it
  * checks the *mathematics*: a mistake shared by the CUDA path and this port is
  * unlikely, and both are pinned against the compiled reference itself

@@ -8,12 +8,11 @@ REPO = Path(__file__).resolve().parent.parent
 sys.path.insert(0, str(REPO))
 
 ORACLE_DIR = REPO / "oracle"
-REF_SO = ORACLE_DIR / "_ref" / "libhbref.so"
 PORT_SO = ORACLE_DIR / "_ref" / "liboracle_port.so"
 
 
 def pytest_configure(config):
-    config.addinivalue_line("markers", "gpu: needs a CUDA device (run on the B200 box)")
+    config.addinivalue_line("markers", "gpu: needs a CUDA device (an H100)")
 
 
 def _have_gpu():
@@ -28,11 +27,9 @@ def _have_gpu():
 
 @pytest.fixture(scope="session")
 def ref():
-    """the reference's own filters (oracle/_ref/libhbref.so), built from /root/reference when present"""
-    from handbrake_b200.hblib import FilterLib
-    if not REF_SO.exists():
-        pytest.skip("oracle/_ref/libhbref.so not built (needs /root/reference at build time)")
-    return FilterLib(REF_SO)
+    """the reference's own filters, answered from their stored result digests (tests/golden_ref.py)"""
+    from golden_ref import GoldenRef
+    return GoldenRef()
 
 
 @pytest.fixture(scope="session")

@@ -2,7 +2,7 @@
 
 oracle/_ref/libhostlogic.so is the PRODUCT's host-side state machine (handbrake_b200/libhb/detelecine_cuda.c,
 compiled untouched) with its device calls redirected to the plain-C restatement oracle/port/detelecine_port.c.  Pinned
-here, frame for frame, against the reference's own hb_filter_detelecine compiled from /root/reference.  On the GPU box the
+here, frame for frame, against the reference's own hb_filter_detelecine (its stored results, tests/golden_ref.py).  On the GPU box the
 same host code drives the CUDA kernels and tests/test_detelecine_gpu.py compares that with the reference."""
 import numpy as np
 import pytest

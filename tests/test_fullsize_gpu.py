@@ -1,5 +1,5 @@
-"""GPU parity at BASELINE.json's full frame sizes (few frames each, so the CPU side finishes in seconds):
-the CUDA filters against the reference itself, bit for bit, plus size-independent properties."""
+"""GPU parity at BASELINE.json's full frame sizes: the CUDA filters against the reference's stored per-frame digests
+(tests/golden_ref.py, digest_only), bit for bit, plus size-independent properties."""
 import numpy as np
 import pytest
 
@@ -11,24 +11,24 @@ FMT = {8: synth.PIX_FMT_YUV420P, 10: synth.PIX_FMT_YUV420P10}
 
 
 def same(r, g):
-    assert g.frames.shape == r.frames.shape
-    if not np.array_equal(g.frames, r.frames):
-        d = g.frames != r.frames
-        raise AssertionError(f"{np.count_nonzero(d)} bytes differ in frames {np.argwhere(d.any(axis=1)).ravel()[:8]}")
+    assert g.frames.shape == r.shape
+    bad = r.frames_differing(g.frames)
+    if bad:
+        raise AssertionError(f"frames {bad[:8]} differ from the reference's")
     assert np.array_equal(g.start, r.start) and list(g.combed) == list(r.combed)
 
 
 def test_config2_1080p_nlmeans_medium(ref, cuda_filters):
     w, h = 1920, 1080
     clip = synth.progressive_clip(FMT[8], w, h, 5)
-    same(ref.run("hb_filter_nlmeans", "y-strength=6:threads=5", clip, FMT[8], w, h),
+    same(ref.run("hb_filter_nlmeans", "y-strength=6:threads=5", clip, FMT[8], w, h, digest_only=True),
          cuda_filters.run("hb_filter_nlmeans_cuda", "y-strength=6", clip, FMT[8], w, h))
 
 
 def test_config4_4k_nlmeans_strong(ref, cuda_filters):
     w, h = 3840, 2160
     clip = synth.progressive_clip(FMT[8], w, h, 4)
-    r = ref.run("hb_filter_nlmeans", "y-strength=10:threads=4", clip, FMT[8], w, h)
+    r = ref.run("hb_filter_nlmeans", "y-strength=10:threads=4", clip, FMT[8], w, h, digest_only=True)
     g = cuda_filters.run("hb_filter_nlmeans_cuda", "y-strength=10", clip, FMT[8], w, h)
     same(r, g)
     # property: denoising shrinks the frame-to-frame noise energy but keeps the mean level
@@ -40,7 +40,7 @@ def test_config4_4k_nlmeans_strong(ref, cuda_filters):
 def test_4k_10bit_nlmeans_medium(ref, cuda_filters):
     w, h = 3840, 2160
     clip = synth.progressive_clip(FMT[10], w, h, 3)
-    same(ref.run("hb_filter_nlmeans", "y-strength=6:threads=3", clip, FMT[10], w, h),
+    same(ref.run("hb_filter_nlmeans", "y-strength=6:threads=3", clip, FMT[10], w, h, digest_only=True),
          cuda_filters.run("hb_filter_nlmeans_cuda", "y-strength=6", clip, FMT[10], w, h))
 
 
@@ -49,7 +49,7 @@ def test_4k_nlmeans_large_window(ref, cuda_filters):
     w, h = 3840, 2160
     clip = synth.progressive_clip(FMT[8], w, h, 5)[:, :]
     s = "y-strength=10:y-origin-tune=0.15:y-patch-size=5:y-range=7:y-frame-count=4"
-    r = ref.run("hb_filter_nlmeans", s + ":threads=5", clip[:3], FMT[8], w, h)
+    r = ref.run("hb_filter_nlmeans", s + ":threads=5", clip[:3], FMT[8], w, h, digest_only=True)
     g = cuda_filters.run("hb_filter_nlmeans_cuda", s, clip[:3], FMT[8], w, h)
     same(r, g)
 
@@ -59,7 +59,7 @@ def test_config3_4k_10bit_comb_detect_decomb_eedi2bob(ref, cuda_filters):
     clip, flags, _ = decomb_inputs(10, w, h, 2, seed=21)          # 2 interlaced + 3 progressive-noise frames
     s = ["mode=3:spatial-metric=2:motion-thresh=1:spatial-thresh=1:filter-mode=2:block-thresh=40:block-width=16:block-height=16",
          "mode=63"]                                                # eedi2bob (31) + selective (32), as work.c sets it
-    r = ref.run(["hb_filter_comb_detect", "hb_filter_decomb"], s, clip, FMT[10], w, h, flags=flags)
+    r = ref.run(["hb_filter_comb_detect", "hb_filter_decomb"], s, clip, FMT[10], w, h, flags=flags, digest_only=True)
     g = cuda_filters.run(["hb_filter_comb_detect_cuda", "hb_filter_decomb_cuda"], s, clip, FMT[10], w, h, flags=flags)
     same(r, g)
     assert g.vrate == (60000, 1001)
@@ -86,7 +86,7 @@ def test_config3_4k_10bit_comb_detect_decomb_eedi2bob(ref, cuda_filters):
 def test_4k_lapsharp(ref, cuda_filters):
     w, h = 3840, 2160
     clip = synth.progressive_clip(FMT[10], w, h, 3, noise=20)
-    same(ref.run("hb_filter_lapsharp", "y-strength=0.2:y-kernel=isolap", clip, FMT[10], w, h),
+    same(ref.run("hb_filter_lapsharp", "y-strength=0.2:y-kernel=isolap", clip, FMT[10], w, h, digest_only=True),
          cuda_filters.run("hb_filter_lapsharp_cuda", "y-strength=0.2:y-kernel=isolap", clip, FMT[10], w, h))
 
 
@@ -99,7 +99,7 @@ def test_config5_8k_10bit_chain(ref, cuda_filters):
     names_r = ["hb_filter_decomb", "hb_filter_nlmeans", "hb_filter_lapsharp_mt"]
     names_g = ["hb_filter_decomb_cuda", "hb_filter_nlmeans_cuda", "hb_filter_lapsharp_cuda"]
     s = ["mode=7", "y-strength=6", "y-strength=0.2:y-kernel=isolap"]
-    r = ref.run(names_r, [s[0], s[1] + ":threads=3", s[2]], clip, FMT[10], w, h, flags=flags)
+    r = ref.run(names_r, [s[0], s[1] + ":threads=3", s[2]], clip, FMT[10], w, h, flags=flags, digest_only=True)
     g = cuda_filters.run(names_g, s, clip, FMT[10], w, h, flags=flags)
     same(r, g)
     assert g.frames.shape[0] == 3

@@ -3,7 +3,7 @@ tables, look-ahead buffering, EOF flush, output order and properties).
 
 oracle/_ref/libhostlogic.so is handbrake_b200/libhb/*_cuda.c compiled UNTOUCHED, with every hbcu_* device call renamed to
 a plain-C stand-in built on the restatement (oracle/port/hostlogic_*.c).  Compared here with the reference's own filter
-objects compiled from /root/reference.  On the GPU box the same host code drives the CUDA kernels (tests/test_*_gpu.py)."""
+objects (their stored results, tests/golden_ref.py).  On the GPU the same host code drives the CUDA kernels (tests/test_*_gpu.py)."""
 import ctypes as C
 import hashlib
 import json

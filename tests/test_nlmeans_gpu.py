@@ -139,8 +139,8 @@ def test_both_ssd_formulations(ref, cuda_filters, monkeypatch, ssd):
 
 @pytest.mark.parametrize("fmt", [FMT8, FMT10])
 def test_round1_kernels_still_agree(ref, cuda_filters, monkeypatch, fmt):
-    """HBCU_NLMEANS_V3=off selects the round-1 fused kernels (nlmeans_fast8 / fast16), the baseline of the v3 levers in
-    profiles/r02b_v3_shape_sweep.txt: they stay bit-exact"""
+    """HBCU_NLMEANS_V3=off selects the round-1 fused kernels (nlmeans_fast8 / fast16), the baseline of the v3 kernels:
+    they stay bit-exact"""
     monkeypatch.setenv("HBCU_NLMEANS_V3", "off")
     w, h = 330, 210
     clip = synth.progressive_clip(fmt, w, h, 4, seed=33)

@@ -1,7 +1,7 @@
 """GPU parity of multi-device dealing: hb_filter_nlmeans_cuda with `devices=...` vs its own single-device run and vs the
 reference (bit-exact).  `devices=0,0` deals the ordered stream to TWO handles on one GPU -- every piece of the path
 (owners, per-device index spaces, halo by device-to-device copy, event ordering between the handles, in-order harvest)
-runs on a 1-GPU box; `devices=0,1` runs when a second GPU is visible (gpurun --gpus 2; NVLink peer copy).
+runs on a 1-GPU box; `devices=0,1` runs when a second GPU is visible (NVLink peer copy).
 VERDICT r1 item 4; the reference's frame-parallel dealing is mt_frame_filter.c:169-237."""
 import ctypes as C
 
@@ -67,7 +67,7 @@ def test_long_stream_many_blocks(cuda_filters):
 def test_two_gpus_equal_one(ref, cuda_filters, settings, block):
     """config 1 over two real devices == one device == the reference (the halo crosses NVLink)"""
     if device_count() < 2:
-        pytest.skip("needs two GPUs (gpurun --gpus 2)")
+        pytest.skip("needs two GPUs")
     w, h, n = 640, 360, 21
     clip = synth.progressive_clip(FMT8, w, h, n, seed=12)
     one = cuda_filters.run("hb_filter_nlmeans_cuda", settings, clip, FMT8, w, h)

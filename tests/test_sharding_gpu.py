@@ -1,7 +1,7 @@
 """GPU: frame-sharded runs of the CUDA filter objects == their unsharded run == the reference (SURVEY.md 8e; VERDICT r1
 (e)(iv): round 1 checked comb-detect / decomb / lapsharp sharding with the CPU objects only).  Every block is a fresh
 filter instance on the device, fed its frames plus the temporal halo of handbrake_b200.sharding; halo outputs are
-dropped.  With two GPUs visible (gpurun --gpus 2) consecutive blocks alternate between them (HBCU_DEVICE)."""
+dropped.  With two GPUs visible consecutive blocks alternate between them (HBCU_DEVICE)."""
 import ctypes as C
 import os
 

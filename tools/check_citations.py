@@ -1,11 +1,12 @@
 """Checks that every `file.c:line[-line]` citation of the reference in this repo points inside an existing file of
-/root/reference/libhb (build container only; the GPU box has no reference).  usage: python tools/check_citations.py"""
+$HANDBRAKE_SRC/libhb (a HandBrake source tree).  usage: python tools/check_citations.py"""
+import os
 import re
 import sys
 from pathlib import Path
 
 REPO = Path(__file__).resolve().parent.parent
-REF = Path("/root/reference/libhb")
+REF = Path(os.environ.get("HANDBRAKE_SRC", ".")) / "libhb"
 PAT = re.compile(r"\b((?:handbrake/|templates/|platform/macosx/)?[A-Za-z0-9_]+\.[ch]):(\d+)(?:-(\d+))?")
 
 

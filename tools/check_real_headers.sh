@@ -1,5 +1,5 @@
 #!/bin/bash
-# Syntax-only compile of the product's host filter sources against the REAL libhb headers in /root/reference/libhb
+# Syntax-only compile of the product's host filter sources against the REAL libhb headers of a HandBrake tree (argument: its libhb directory)
 # (not the test shim in handbrake_b200/libhb/handbrake/), backing INTEGRATION.md's claim that they drop into a HandBrake
 # tree unchanged.  libav*/jansson are replaced by type-only stubs (tools/real_header_stubs/), project.h by a stand-in
 # with every optional feature off.  What is NOT in the real tree and therefore shows up here is exactly the integration
@@ -7,7 +7,7 @@
 # (hb_shim_set_frame_allocator / hb_shim_set_device_release / hb_shim_set_device_retain).
 # usage: tools/check_real_headers.sh [reference libhb dir]      exit 0 = no errors
 export LC_ALL=C
-REF=${1:-/root/reference/libhb}
+REF=${1:?usage: check_real_headers.sh <HandBrake tree>/libhb}
 REPO=$(cd "$(dirname "$0")/.." && pwd)
 [ -d "$REF/handbrake" ] || { echo "no reference tree at $REF"; exit 2; }
 TMP=$(mktemp -d)

@@ -1,6 +1,6 @@
-// latency_bench.cu -- dependent-issue latencies of one warp on sm_100a (what bounds hqdn3d's lookup chains) and the
+// latency_bench.cu -- dependent-issue latencies of one warp on sm_90a (what bounds hqdn3d's lookup chains) and the
 // throughput of the fp64 conversion / multiply instructions lapsharp's sharpening expression needs.
-//   nvcc -gencode arch=compute_100a,code=sm_100a -O3 -o latency_bench tools/latency_bench.cu && ./latency_bench
+//   nvcc -gencode arch=compute_90a,code=sm_90a -O3 -o latency_bench tools/latency_bench.cu && ./latency_bench
 #include <cstdio>
 #include <cstdint>
 #include <cuda_runtime.h>
@@ -74,8 +74,8 @@ int main()
     {
         chain<0><<<1, 32>>>(dt, out, cyc, 2); chain<1><<<1, 32>>>(dt, out, cyc, 2); chain<2><<<1, 32>>>(dt, out, cyc, 2);
         chain<3><<<1, 32>>>(dt, out, cyc, 2); chain<4><<<1, 32>>>(dt, out, cyc, 2); chain<5><<<1, 32>>>(dt, out, cyc, 3);
-        fp64_rate<0><<<148, 1024>>>(out, cyc, 1); fp64_rate<1><<<148, 1024>>>(out, cyc, 1);
-        fp64_rate<2><<<148, 1024>>>(out, cyc, 1); fp64_rate<3><<<148, 1024>>>(out, cyc, 1);
+        fp64_rate<0><<<132, 1024>>>(out, cyc, 1); fp64_rate<1><<<132, 1024>>>(out, cyc, 1);
+        fp64_rate<2><<<132, 1024>>>(out, cyc, 1); fp64_rate<3><<<132, 1024>>>(out, cyc, 1);
         cudaDeviceSynchronize();
     }
     const char *names[6] = { "LDS->LDS", "LDS,IADD,SHF,LOP", "LDS,IADD,IADD,SHF,LOP", "IADD", "SHF,LOP", "IMAD" };

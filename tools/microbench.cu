@@ -24,9 +24,6 @@ __device__ __forceinline__ void body(uint32_t (&r)[NCH], uint32_t k0, uint32_t k
 DEF_OP32(0,  "add.rn.f32 %0, %0, %1;")
 DEF_OP32(1,  "mul.rn.f32 %0, %0, %1;")
 DEF_OP32(2,  "fma.rn.f32 %0, %0, %1, %2;")
-DEF_OP64(3,  "add.rn.f32x2 %0, %0, %1;")
-DEF_OP64(4,  "mul.rn.f32x2 %0, %0, %1;")
-DEF_OP64(5,  "fma.rn.f32x2 %0, %0, %1, %1;")
 DEF_OP32(6,  "add.u32 %0, %0, %1;")
 DEF_OP32(7,  "mad.lo.u32 %0, %0, %1, %2;")
 DEF_OP32(8,  "lop3.b32 %0, %0, %1, %2, 0x96;")
@@ -53,20 +50,13 @@ DEF_OP32(27, "add.rn.f32 %0, %0, %1; prmt.b32 %0, %0, %1, 0x4321;")        // FA
 
 
 // independent mixes: the first half of the chains runs op A, the second half op B (no dependency between them) --
-// which pairs overlap says which pipe each instruction sits on and whether a packed f32x2 costs one issue slot or two
+// which pairs overlap says which pipe each instruction sits on
 #define DEF_MIX32(ID, ASMA, ASMB)                                                             \
     template <> __device__ __forceinline__ void body<ID>(uint32_t (&r)[NCH], uint32_t k0,     \
         uint32_t k1, uint64_t (&q)[NCH], float *sm, int lane) {                               \
         _Pragma("unroll") for (int i = 0; i < NCH / 2; i++) {                                 \
             asm volatile(ASMA : "+r"(r[i]) : "r"(k0), "r"(k1));                               \
             asm volatile(ASMB : "+r"(r[i + NCH / 2]) : "r"(k0), "r"(k1)); } }
-#define DEF_MIX64(ID, ASMA, ASMB)                                                             \
-    template <> __device__ __forceinline__ void body<ID>(uint32_t (&r)[NCH], uint32_t k0,     \
-        uint32_t k1, uint64_t (&q)[NCH], float *sm, int lane) {                               \
-        uint64_t kk = ((uint64_t)k1 << 32) | k0;                                              \
-        _Pragma("unroll") for (int i = 0; i < NCH; i++) {                                     \
-            asm volatile(ASMA : "+l"(q[i]) : "l"(kk));                                        \
-            asm volatile(ASMB : "+r"(r[i]) : "r"(k0), "r"(k1)); } }
 #define A_FFMA  "fma.rn.f32 %0, %0, %1, %2;"
 #define A_LOP3  "lop3.b32 %0, %0, %1, %2, 0x96;"
 #define A_DP4A  "dp4a.u32.u32 %0, %0, %1, %2;"
@@ -75,10 +65,6 @@ DEF_OP32(27, "add.rn.f32 %0, %0, %1; prmt.b32 %0, %0, %1, 0x4321;")        // FA
 #define A_PRMT  "prmt.b32 %0, %0, %1, 0x4321;"
 #define A_IMAD  "mad.lo.u32 %0, %0, %1, %2;"
 #define A_SHF   "shf.l.wrap.b32 %0, %0, %1, %2;"
-DEF_MIX64(40, "fma.rn.f32x2 %0, %0, %1, %1;", A_LOP3)
-DEF_MIX64(41, "fma.rn.f32x2 %0, %0, %1, %1;", A_FFMA)
-DEF_MIX64(42, "add.rn.f32x2 %0, %0, %1;", A_DP4A)
-DEF_MIX64(43, "add.rn.f32x2 %0, %0, %1;", A_PRMT)
 DEF_MIX32(44, A_DP4A, A_LOP3)
 DEF_MIX32(45, A_DP4A, A_FFMA)
 DEF_MIX32(46, A_VABS, A_DP4A)
@@ -147,11 +133,13 @@ __global__ void __launch_bounds__(1024, 1) bench(uint32_t *out, long long *cycle
     if (threadIdx.x == 0) cycles[blockIdx.x] = t1 - t0;
 }
 
+static int g_nblk = 1;
+
 template <int OP>
 void run(const char *name, int ptx_per_body, int nthreads = 1024)
 {
     uint32_t *out; long long *cyc;
-    int nblk = 148;
+    const int nblk = g_nblk;                         // one block per SM
     cudaMalloc(&out, nblk * 1024 * 4); cudaMalloc(&cyc, nblk * 8);
     size_t smem = (128 * 32 + 4096) * 4;
     cudaFuncSetAttribute(bench<OP>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
@@ -162,7 +150,7 @@ void run(const char *name, int ptx_per_body, int nthreads = 1024)
     cudaEventRecord(e1);
     cudaError_t err = cudaDeviceSynchronize();
     float ms; cudaEventElapsedTime(&ms, e0, e1);
-    long long h[148]; cudaMemcpy(h, cyc, nblk * 8, cudaMemcpyDeviceToHost);
+    long long h[1024]; cudaMemcpy(h, cyc, nblk * 8, cudaMemcpyDeviceToHost);
     double avg = 0; for (int i = 0; i < nblk; i++) avg += h[i]; avg /= nblk;
     double winstr = (double)(nthreads / 32) * ITER * NCH * ptx_per_body;
     printf("%-28s thr=%4d cycles=%9.0f  warp-instr/clk/SM=%6.3f  (lane-ops/clk/SM=%7.1f)  ms=%.3f %s\n", name, nthreads, avg,
@@ -174,8 +162,8 @@ int main()
 {
     cudaDeviceProp p; cudaGetDeviceProperties(&p, 0);
     printf("device %s  SMs=%d  clock=%d kHz\n", p.name, p.multiProcessorCount, p.clockRate);
+    g_nblk = p.multiProcessorCount < 1024 ? p.multiProcessorCount : 1024;
     run<0>("FADD", 1); run<1>("FMUL", 1); run<2>("FFMA", 1);
-    run<3>("FADD2 (f32x2)", 1); run<4>("FMUL2 (f32x2)", 1); run<5>("FFMA2 (f32x2)", 1);
     run<6>("IADD", 1); run<7>("IMAD", 1); run<8>("LOP3", 1); run<9>("PRMT", 1); run<10>("FMNMX", 1);
     run<11>("I2F.S32", 1); run<12>("F2I.RZ", 1); run<13>("IDP4A", 1); run<14>("VABSDIFF4", 1);
     run<15>("FADD.RZ", 1); run<16>("FMUL.SAT", 1); run<17>("FSETP+SEL", 2); run<18>("SHF", 1);
@@ -184,12 +172,11 @@ int main()
     run<24>("mix FADD+IADD", 2); run<25>("mix FFMA+LOP3", 2); run<26>("mix FFMA+IMAD", 2); run<27>("mix FADD+PRMT", 2);
     run<30>("LDS.32 (+LOP)", 1); run<31>("LDS.128 (+3LOP)", 1); run<32>("LDS.32 LUT replicated", 1);
     run<33>("LDS.32 LUT 128-entry", 1); run<34>("LDS.64+STS.64 RMW", 2);
-    run<40>("ind FFMA2 | LOP3", 2); run<41>("ind FFMA2 | FFMA", 2); run<42>("ind FADD2 | IDP4A", 2); run<43>("ind FADD2 | PRMT", 2);
     run<44>("ind IDP4A | LOP3", 1); run<45>("ind IDP4A | FFMA", 1); run<46>("ind VABSDIFF4 | IDP4A", 1); run<47>("ind VABSDIFF4 | LOP3", 1);
     run<48>("ind VABSDIFF4 | FFMA", 1); run<49>("ind IADD3 | FFMA", 1); run<50>("ind IADD3 | LOP3", 1); run<51>("ind IADD3 | IDP4A", 1);
     run<52>("ind PRMT | LOP3", 1); run<53>("ind IMAD | IDP4A", 1); run<54>("ind SHF | LOP3", 1); run<55>("ind SHF | FFMA", 1);
     run<56>("ind FFMA | LOP3", 1); run<57>("ind IADD3 | IADD3", 1);
     // occupancy sensitivity of the FP pipe
-    run<0>("FADD", 1, 512); run<0>("FADD", 1, 256); run<2>("FFMA", 1, 256); run<5>("FFMA2", 1, 256);
+    run<0>("FADD", 1, 512); run<0>("FADD", 1, 256); run<2>("FFMA", 1, 256);
     return 0;
 }

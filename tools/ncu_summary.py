@@ -2,7 +2,7 @@
 """tools/ncu_summary.py REPORT.ncu-rep [--kernel REGEX] [--capture TEXT] [--workload TEXT] [--alg-bytes N] [--note K=V ...]
 
 Reads an `ncu --set full` report (here, no GPU needed: `ncu -i ... --page raw --csv`) and prints the JSON summary that is
-committed under profiles/ and that bench.py reads for `roofline.traffic` / `roofline.issue_frac`."""
+that bench.py can read for `roofline.traffic` / `roofline.issue_frac`."""
 import argparse
 import csv
 import io

@@ -1,8 +1,7 @@
 #!/usr/bin/env python
-"""tools/sass_excerpt.py [libhbcu.so] -- per-kernel SASS evidence for profiles/: architecture of every cubin, and for each
+"""tools/sass_excerpt.py [libhbcu.so] -- per-kernel SASS evidence: architecture of every cubin, and for each
 kernel the instruction mnemonics that prove how it moves data and does its arithmetic (TMA: UTMALDG + mbarrier SYNCS;
-tensor memory: LDTM/STTM + the UTCATOMSWS allocation; packed bytes: VABSDIFF4/IDP; packed fp32 pairs: FADD2/FFMA2;
-vector loads; FP64), with the first occurrence of each as an excerpt line."""
+packed bytes: VABSDIFF4/IDP; vector loads; FP64), with the first occurrence of each as an excerpt line."""
 import collections
 import re
 import subprocess
@@ -13,7 +12,7 @@ so = sys.argv[1] if len(sys.argv) > 1 else str(Path(__file__).resolve().parent.p
 txt = subprocess.run(["cuobjdump", "-sass", so], capture_output=True, text=True).stdout
 arch = collections.Counter(re.findall(r"arch = (sm_\w+)", txt))
 print(f"# {Path(so).name}: cubins by architecture: {dict(arch)}")
-WATCH = ["UTMALDG", "SYNCS", "LDTM", "STTM", "UTCATOMSWS", "VABSDIFF4", "IDP", "FADD2", "FFMA2", "LDG.E.128", "LDS.128", "LDG.E.64", "STG.E.128",
+WATCH = ["UTMALDG", "SYNCS", "VABSDIFF4", "IDP", "LDG.E.128", "LDS.128", "LDG.E.64", "STG.E.128",
          "DADD", "DMUL", "DFMA", "SHFL", "ATOM", "RED", "MUFU", "LDGSTS"]
 cur, body = None, []
 
