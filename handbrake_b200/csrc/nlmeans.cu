@@ -1620,7 +1620,7 @@ constexpr int kTH8 = 144;
 int g_ssd_variant = 1;     // 1: packed-byte VABSDIFF4 + IDP4A patch-row sums (measured 7 % faster), 0: fp32 prefix sums (FFMA);
                            // HBCU_NLMEANS_SSD selects (test/tuning hook: both are exact, tests run both)
 
-template <int NH, int NW, int RS, int NBUF>
+template <int NH, int NW, int RS, int NBUF, bool SYM = false>
 int launch_v3(FusedParams &fp, cudaStream_t st)
 {
     using L = V3Layout<NW, RS, NBUF>;
@@ -1632,7 +1632,7 @@ int launch_v3(FusedParams &fp, cudaStream_t st)
     bool &configured = configured_on[dev_ & (kMaxDevices - 1)];
     if (!configured)
     {
-        HBCU_CHECK(cudaFuncSetAttribute(nlmeans_v3_kernel<NH, NW, RS, NBUF>, cudaFuncAttributeMaxDynamicSharedMemorySize, L::kTotal));
+        HBCU_CHECK(cudaFuncSetAttribute(nlmeans_v3_kernel<NH, NW, RS, NBUF, false, SYM>, cudaFuncAttributeMaxDynamicSharedMemorySize, L::kTotal));
         configured = true;
     }
     int total = 0;
@@ -1643,7 +1643,7 @@ int launch_v3(FusedParams &fp, cudaStream_t st)
         total += fp.tiles_x[i] * ((fp.k[i].h + L::kTH - 1) / L::kTH);
     }
     fp.first_tile[fp.nplanes] = total;
-    nlmeans_v3_kernel<NH, NW, RS, NBUF><<<total, NW * 32, L::kTotal, st>>>(fp);
+    nlmeans_v3_kernel<NH, NW, RS, NBUF, false, SYM><<<total, NW * 32, L::kTotal, st>>>(fp);
     hbcu::count_launch();
     return 0;
 }
@@ -1753,6 +1753,15 @@ int launch_v3_nh(int nw, int rs, FusedParams &fp, cudaStream_t st)
             if (!v3_group_known(ng, (12 + dx0) & 3, kOrgNone)) return 1;
             if (dx0 <= 0 && dx0 + ng > 0 && !v3_group_known(ng, (12 + dx0) & 3, -dx0)) return 1;
         }
+    // range 3 in every plane: frame 0 runs as one symmetric march (V3Sym, nlmeans_v3.cuh)
+    bool sym = true;
+    for (int pl = 0; pl < fp.nplanes; pl++) sym = sym && fp.k[pl].r_half == 1;
+    if (sym && nw == 12 && rs == 10)
+    {
+        if (nh == 1) return launch_v3<1, 12, 10, 2, true>(fp, st);
+        if (nh == 2) return launch_v3<2, 12, 10, 2, true>(fp, st);
+        if (nh == 3) return launch_v3<3, 12, 10, 2, true>(fp, st);
+    }
 #define V3CASE(NH_, NW_, RS_, NB_) if (nh == NH_ && nw == NW_ && rs == RS_) return launch_v3<NH_, NW_, RS_, NB_>(fp, st)
     V3CASE(1, 12, 10, 2); V3CASE(2, 12, 10, 2); V3CASE(3, 12, 10, 2);
     V3CASE(4, 8, 15, 2);

@@ -16,7 +16,10 @@
 //   * the compare tile of frame 1 is in flight while frame 0 is compared with itself (second mbarrier);
 //   * accumulators (weight sum, pixel sum; 8 bytes per pixel) live in shared memory, a float4 per lane and array and row.
 //     Together with the tiles they bound the tile height: 120 rows (12 warps x 10) keep the largest variant (16-bit
-//     tiles, or the four tiles of the prefilter variant) inside the 227 KB an H100 block can have.
+//     tiles, or the four tiles of the prefilter variant) inside the 227 KB an H100 block can have;
+//   * range 3 without a prefilter (the SYM instantiation): frame 0, the current frame compared with itself, is one march
+//     over four displacements instead of three over eight -- the other four weights are the same floats read one column
+//     left or one row up (V3Sym) -- and it stores the accumulators instead of adding to zero-filled ones.
 #pragma once
 
 template <int NW, int RS, int NBUF, int BPS = 1, bool PRE = false>
@@ -395,9 +398,261 @@ __host__ __device__ inline bool v3_group_known(int ng, int ob, int org)
     return false;
 }
 
-template <int NH, int NW, int RS, int NBUF, bool PRE = false>
+// Frame 0 of a range-3 search (r_half == 1) in one march.  Frame 0 compares the current tile with itself, and there the
+// patch distance is symmetric: SSD_{-d}(p) == SSD_d(p - d), the same integer from the same tile bytes, so the weight
+// (a function of that integer alone) is the same float.  Four "forward" displacements give all eight weights:
+//   A = (0,+1), B = (+1,+1), C = (+1,0), D = (+1,-1);
+//   (0,-1) at x is A at x-1;  (-1,-1) at (y, x) is B at (y-1, x-1);  (-1,0) is C at (y-1, x);  (-1,+1) is D at (y-1, x+1).
+// A lane keeps the running sums of A and B at columns x-1 .. x+3, C at x .. x+3 and D at x .. x+4 (the windows at x-1
+// and x+4 come out of the same D words as the lane's own four: no shuffles), starting one row above the strip so that
+// row -1 has (+1, .) weights.  The weights of the (+1, .) displacements are kept for one row; the patch-row sum leaving
+// a running sum is recomputed from the tile instead of kept (a 2NH+1-row history of 19 sums does not fit the register
+// budget of 12 warps).  The nine frame-0 terms of an output pixel are added in registers in the reference's order --
+// (-1,-1) (-1,0) (-1,1) (0,-1) origin (0,1) (1,-1) (1,0) (1,1) -- one IEEE operation each, as V3Group does, and stored
+// with plain stores: the accumulators need no zero fill.  The first term is stored as is (0 + w == w, 0 + w*p == w*p:
+// weights and pixels are never negative).
+//
+// Row slots: output row r (r = -1 .. rows-1) runs in slot K = (r + 1) % 6.  Its compare-row words are kept by parity
+// (the words of row t + 1 are the source words of the next step), its pixel rows by row mod 3: every array index is a
+// compile-time constant of the unrolled slot.
+template <int NH, class ACC>
+struct V3Sym
+{
+    static constexpr int PW = kTilePW / 4;           // tile pitch in words
+    static_assert(NH >= 1 && NH <= 3, "patch size");
+
+    uint32_t VA[5], VB[5], VC[4], VD[5];             // 2^23-biased running sums; A, B: columns x-1 .. x+3, C: x .. x+3, D: x .. x+4
+    uint32_t qi[2][5], qo[2][5];                     // words lane+2 .. lane+6 of the compare row entering / leaving the sums
+    float pix[3][6];                                 // pixels x-1 .. x+4 of a row, as floats
+    float WB[2][5], WC[2][4], WD[2][5];              // weights of the (+1, .) displacements, same columns as their sums
+    const uint32_t *base;                            // tile word `lane` of output row 0
+    const ACC &acc;
+    uint32_t lut_lane_addr;
+    float wscale, wbias;
+    double origin_tune;
+
+    __device__ __forceinline__ V3Sym(const uint32_t *cur, const ACC &acc_, uint32_t lut_lane_addr_, float wscale_, float wbias_,
+                                     double origin_tune_, int seg_y0, int lane)
+        : acc(acc_), lut_lane_addr(lut_lane_addr_), wscale(wscale_), wbias(wbias_), origin_tune(origin_tune_)
+    {
+        base = cur + (seg_y0 + kHalo) * PW + lane;
+    }
+
+    // patch-row sum of window I (columns x+I-NH .. x+I+NH) from the D words of a row (byte j: column x-4+j); T[w] is
+    // IDP4A(D[w], D[w])
+    template <int I>
+    static __device__ __forceinline__ uint32_t window(const uint32_t (&D)[3], const uint32_t (&T)[3])
+    {
+        constexpr int b0 = 4 - NH + I, b1 = 4 + NH + I;
+        static_assert(b0 >= 0 && b1 <= 11, "window outside the D words");
+        if constexpr (NH == 3 && I >= 0 && I <= 3)
+        {
+            // V3Group's patch-7 form: bytes 4..7 shared, the other three gathered into one word (byte 0 cleared)
+            const uint32_t Z = D[0] & 0xFFFFFF00u;
+            const uint32_t X = I == 0 ? Z : __byte_perm(Z, D[2], I == 1 ? 0x0432 : I == 2 ? 0x0543 : 0x0654);
+            return __dp4a(X, X, T[1]);
+        }
+        else
+        {
+            int full = -1;                           // the first whole word of the window starts the sum
+#pragma unroll
+            for (int w = 0; w < 3; w++)
+                if (full < 0 && b0 <= 4 * w && 4 * w + 3 <= b1) full = w;
+            uint32_t hs = full >= 0 ? T[full] : 0u;
+#pragma unroll
+            for (int w = 0; w < 3; w++)
+            {
+                const int lo = b0 > 4 * w ? b0 : 4 * w, hi = b1 < 4 * w + 3 ? b1 : 4 * w + 3;
+                if (lo > hi || w == full) continue;
+                if (lo == 4 * w && hi == 4 * w + 3) hs = __dp4a(D[w], D[w], hs);
+                else
+                {
+                    uint32_t m = 0;
+#pragma unroll
+                    for (int bb = 0; bb < 4; bb++)
+                        if (4 * w + bb >= lo && 4 * w + bb <= hi) m |= 0xFFu << (8 * bb);
+                    hs = __dp4a(D[w] & m, D[w], hs);
+                }
+            }
+            return hs;
+        }
+    }
+
+    template <int LO, int... Is>
+    static __device__ __forceinline__ void windows(const uint32_t (&D)[3], uint32_t (&hs)[sizeof...(Is)], std::integer_sequence<int, Is...>)
+    {
+        uint32_t T[3];
+#pragma unroll
+        for (int w = 0; w < 3; w++) T[w] = __dp4a(D[w], D[w], 0u);
+        ((hs[Is] = window<LO + Is>(D, T)), ...);
+    }
+
+    // patch-row sums of one row: source words a = lane+3 .. lane+6 of row t, q = lane+2 .. lane+6 of row t+1
+    static __device__ __forceinline__ void row_sums(const uint32_t (&a)[4], const uint32_t (&q)[5],
+                                                    uint32_t (&hA)[5], uint32_t (&hB)[5], uint32_t (&hC)[4], uint32_t (&hD)[5])
+    {
+        uint32_t DA[3], DB[3], DC[3], DD[3];
+#pragma unroll
+        for (int w = 0; w < 3; w++)
+        {
+            DA[w] = __vabsdiffu4(a[w], __funnelshift_r(a[w], a[w + 1], 8));      // row t, one column right
+            DB[w] = __vabsdiffu4(a[w], __funnelshift_r(q[w + 1], q[w + 2], 8));  // row t+1, one column right
+            DC[w] = __vabsdiffu4(a[w], q[w + 1]);                                // row t+1
+            DD[w] = __vabsdiffu4(a[w], __funnelshift_r(q[w], q[w + 1], 24));     // row t+1, one column left
+        }
+        windows<-1>(DA, hA, std::make_integer_sequence<int, 5>{});
+        windows<-1>(DB, hB, std::make_integer_sequence<int, 5>{});
+        windows<0>(DC, hC, std::make_integer_sequence<int, 4>{});
+        windows<0>(DD, hD, std::make_integer_sequence<int, 5>{});
+    }
+
+    // compare row `row` (relative to output row 0) into q[P]; the sums of row - 1, whose source words are q[1 - P]
+    template <int P>
+    __device__ __forceinline__ void sums(uint32_t (&q)[2][5], int row, uint32_t (&hA)[5], uint32_t (&hB)[5], uint32_t (&hC)[4], uint32_t (&hD)[5])
+    {
+#pragma unroll
+        for (int k = 0; k < 5; k++) q[P][k] = base[row * PW + 2 + k];
+        const uint32_t a[4] = { q[1 - P][1], q[1 - P][2], q[1 - P][3], q[1 - P][4] };
+        row_sums(a, q[P], hA, hB, hC, hD);
+    }
+
+    template <int S>
+    __device__ __forceinline__ void load_pixels(int row)
+    {
+        const uint32_t *w = base + row * PW + 3;
+        const uint32_t w0 = w[0], w1 = w[1], w2 = w[2];
+        pix[S][0] = __fadd_rn(byte_as_biased_float(w0, 3), -8388608.0f);
+#pragma unroll
+        for (int i = 0; i < 4; i++) pix[S][1 + i] = __fadd_rn(byte_as_biased_float(w1, i), -8388608.0f);
+        pix[S][5] = __fadd_rn(byte_as_biased_float(w2, 0), -8388608.0f);
+    }
+
+    __device__ __forceinline__ float weight(uint32_t v) const
+    {
+        float t, w;
+        asm("fma.rn.sat.f32 %0, %1, %2, %3;" : "=f"(t) : "f"(__uint_as_float(v)), "f"(wscale), "f"(wbias));
+        const float u = __fadd_rz(t, 65536.0f);                                  // 65536 + floor(128 t)
+        asm("ld.shared.f32 %0, [%1];" : "=f"(w) : "r"((__float_as_uint(u) << 7) + lut_lane_addr));
+        return w;
+    }
+
+    template <int P>
+    __device__ __forceinline__ void plus_weights()
+    {
+#pragma unroll
+        for (int k = 0; k < 5; k++) WB[P][k] = weight(VB[k]);
+#pragma unroll
+        for (int k = 0; k < 4; k++) WC[P][k] = weight(VC[k]);
+#pragma unroll
+        for (int k = 0; k < 5; k++) WD[P][k] = weight(VD[k]);
+    }
+
+    // output row r in slot K
+    template <int K>
+    __device__ __forceinline__ void step(int r)
+    {
+        constexpr int P = K % 2, Q = 1 - P;                                      // this row's and the previous row's weights
+        constexpr int SM = (K + 1) % 3, S0 = (K + 2) % 3, SP = K % 3;           // pixel rows r-1, r, r+1
+        {
+            uint32_t iA[5], iB[5], iC[4], iD[5], oA[5], oB[5], oC[4], oD[5];
+            sums<P>(qi, r + NH + 1, iA, iB, iC, iD);                            // patch row r+NH enters
+            sums<P>(qo, r - NH, oA, oB, oC, oD);                                // patch row r-NH-1 leaves
+#pragma unroll
+            for (int k = 0; k < 5; k++)
+            {
+                VA[k] = VA[k] + iA[k] - oA[k];
+                VB[k] = VB[k] + iB[k] - oB[k];
+                VD[k] = VD[k] + iD[k] - oD[k];
+            }
+#pragma unroll
+            for (int k = 0; k < 4; k++) VC[k] = VC[k] + iC[k] - oC[k];
+        }
+        load_pixels<SP>(r + 1);
+        float WA[5];
+#pragma unroll
+        for (int k = 0; k < 5; k++) WA[k] = weight(VA[k]);
+        plus_weights<P>();
+        uint32_t accv[8];
+#pragma unroll
+        for (int i = 0; i < 4; i++)
+        {
+            const float *pm = pix[SM], *p0 = pix[S0], *pp = pix[SP];
+            float ws = WB[Q][i];                                                  // (-1,-1) = B at (r-1, x+i-1)
+            float ps = __fmul_rn(WB[Q][i], pm[i]);
+            ws = __fadd_rn(ws, WC[Q][i]);                                         // (-1, 0) = C at (r-1, x+i)
+            ps = __fadd_rn(ps, __fmul_rn(WC[Q][i], pm[i + 1]));
+            ws = __fadd_rn(ws, WD[Q][i + 1]);                                     // (-1,+1) = D at (r-1, x+i+1)
+            ps = __fadd_rn(ps, __fmul_rn(WD[Q][i + 1], pm[i + 2]));
+            ws = __fadd_rn(ws, WA[i]);                                            // ( 0,-1) = A at (r, x+i-1)
+            ps = __fadd_rn(ps, __fmul_rn(WA[i], p0[i]));
+            ws = (float)__dadd_rn((double)ws, origin_tune);                       // origin (add_origin)
+            ps = (float)__dadd_rn((double)ps, __dmul_rn(origin_tune, (double)p0[i + 1]));
+            ws = __fadd_rn(ws, WA[i + 1]);                                        // ( 0,+1)
+            ps = __fadd_rn(ps, __fmul_rn(WA[i + 1], p0[i + 2]));
+            ws = __fadd_rn(ws, WD[P][i]);                                         // (+1,-1)
+            ps = __fadd_rn(ps, __fmul_rn(WD[P][i], pp[i]));
+            ws = __fadd_rn(ws, WC[P][i]);                                         // (+1, 0)
+            ps = __fadd_rn(ps, __fmul_rn(WC[P][i], pp[i + 1]));
+            ws = __fadd_rn(ws, WB[P][i + 1]);                                     // (+1,+1)
+            ps = __fadd_rn(ps, __fmul_rn(WB[P][i + 1], pp[i + 2]));
+            accv[v3_acc_slot(i)] = __float_as_uint(ws);
+            accv[4 + v3_acc_slot(i)] = __float_as_uint(ps);
+        }
+        acc.store(r, accv);
+    }
+
+    template <int... Ms>
+    __device__ __forceinline__ void rows_from(int r0, int rows, std::integer_sequence<int, Ms...>)
+    {
+        ((r0 + Ms < rows ? step<(Ms + 1) % 6>(r0 + Ms) : (void)0), ...);
+    }
+
+    // warm-up row j (patch row t = j - NH - 1) adds its sums
+    template <int... Js>
+    __device__ __forceinline__ void warm_up(std::integer_sequence<int, Js...>)
+    {
+        ((warm_row<Js % 2>(Js - NH - 1)), ...);
+    }
+    template <int P>
+    __device__ __forceinline__ void warm_row(int t)
+    {
+        uint32_t hA[5], hB[5], hC[4], hD[5];
+        sums<P>(qi, t + 1, hA, hB, hC, hD);
+#pragma unroll
+        for (int k = 0; k < 5; k++)
+        {
+            VA[k] += hA[k];
+            VB[k] += hB[k];
+            VD[k] += hD[k];
+        }
+#pragma unroll
+        for (int k = 0; k < 4; k++) VC[k] += hC[k];
+    }
+
+    __device__ __forceinline__ void run(int rows)
+    {
+#pragma unroll
+        for (int k = 0; k < 5; k++) VA[k] = VB[k] = VD[k] = kVBias;
+#pragma unroll
+        for (int k = 0; k < 4; k++) VC[k] = kVBias;
+        // source words of patch row -NH-1: the first row of the warm-up, and the first row the march takes out again
+#pragma unroll
+        for (int k = 1; k < 5; k++) qo[0][k] = qi[1][k] = base[(-NH - 1) * PW + 2 + k];
+        // row -1: the sums of patch rows -NH-1 .. NH-1 (the last one leaves its compare words in qi[0]), the (+1, .) weights
+        warm_up(std::make_integer_sequence<int, 2 * NH + 1>{});
+        plus_weights<0>();
+        load_pixels<2>(-1);
+        load_pixels<0>(0);
+#pragma unroll 1
+        for (int r0 = 0; r0 < rows; r0 += 6) rows_from(r0, rows, std::make_integer_sequence<int, 6>{});
+        acc.wait_store();
+    }
+};
+
+template <int NH, int NW, int RS, int NBUF, bool PRE = false, bool SYM = false>
 __global__ void __launch_bounds__(NW * 32, 1) nlmeans_v3_kernel(const __grid_constant__ FusedParams fp)
 {
+    static_assert(!SYM || (!PRE && NH <= 3), "the symmetric frame-0 march: no prefilter, patch 3 .. 7");
     constexpr int kThreads = NW * 32;
     using L = V3Layout<NW, RS, NBUF, 1, PRE>;
     int pl = 0;
@@ -447,14 +702,17 @@ __global__ void __launch_bounds__(NW * 32, 1) nlmeans_v3_kernel(const __grid_con
     const int seg_y0 = warp * RS;
     int rows = p.h - (Y0 + seg_y0);                                     // rows of this warp's strip inside the plane
     rows = rows < 0 ? 0 : (rows > RS ? RS : rows);
+    // range 3 without prefilter: frame 0 is one symmetric march (V3Sym) that stores every accumulator row it owns
+    const bool sym = SYM && p.r_half == 1;
     V3Acc acc;
     float *acc_ws = reinterpret_cast<float *>(smem + L::kOffWs);
     float *acc_ps = reinterpret_cast<float *>(smem + L::kOffPs);
-    for (int i = tid; i < L::kTH * kTileW; i += kThreads)
-    {
-        acc_ws[i] = 0.f;
-        acc_ps[i] = 0.f;
-    }
+    if (!sym)
+        for (int i = tid; i < L::kTH * kTileW; i += kThreads)
+        {
+            acc_ws[i] = 0.f;
+            acc_ps[i] = 0.f;
+        }
     acc.ws = acc_ws + seg_y0 * kTileW + lane * 4;
     acc.ps = acc_ps + seg_y0 * kTileW + lane * 4;
     mbar_wait(bar, 0);
@@ -480,10 +738,19 @@ __global__ void __launch_bounds__(NW * 32, 1) nlmeans_v3_kernel(const __grid_con
         }
         // the tile the patch distances compare against: the pre-denoised twin of `bw` in the prefilter variant
         const uint32_t *bd = !PRE ? bw : (f == 0 ? pre0w : reinterpret_cast<const uint32_t *>(smem + L::kOffCmpPre));
+        constexpr bool kExact = RS % (2 * NH + 1) == 0;                 // then partial strips run to their end (rows beyond the plane are never stored)
+        const int nrows = kExact ? RS : rows;
+        if constexpr (SYM)
+        {
+            if (sym && f == 0)
+            {
+                // every row the later frames' marches read and write (nrows) is stored here
+                if (rows > 0) V3Sym<NH, V3Acc>(cw, acc, lut_lane_addr, wscale, wbias, p.origin_tune, seg_y0, lane).run(nrows);
+                continue;
+            }
+        }
         if (rows > 0)
         {
-            constexpr bool kExact = RS % (2 * NH + 1) == 0;             // then partial strips run to their end (rows beyond the plane are never stored)
-            const int nrows = kExact ? RS : rows;
             for (int dy = -p.r_half; dy <= p.r_half; dy++)
             {
                 for (int dx0 = -p.r_half; dx0 <= p.r_half; dx0 += kGroup)
