@@ -2110,12 +2110,17 @@ int run_filter(hbcu_nlmeans_s *h, int64_t index, int navail, int oslot, void *co
             for (int f = 0; f < kps[pl].nf; f++) fp.maps[fp.nplanes][f] = (v3 ? h->maps3 : h->maps)[slots[pl][f] * 3 + pl];
             fp.nplanes++;
         }
-        if ((v3 ? launch_v3_nh(vs.nw, vs.rs, fp, h->s_compute) : launch_fast8_nh(fp, h->s_compute)) != 0)
-        { set_error("nlmeans: fused launch failed"); return -1; }
-        HBCU_CHECK(cudaGetLastError());
-        h->kernel_launches++;
+        const int rc8 = v3 ? launch_v3_nh(vs.nw, vs.rs, fp, h->s_compute) : launch_fast8_nh(fp, h->s_compute);
+        if (rc8 < 0) { set_error("nlmeans: fused launch failed"); return -1; }
+        if (rc8 == 0)
+        {
+            HBCU_CHECK(cudaGetLastError());
+            h->kernel_launches++;
+        }
+        // a range the v3 group shapes do not cover (range 1): one launch per plane, as launch_plane() picks for it
+        else fused = false;
     }
-    else
+    if (!(fused16 && nact > 0) && !(fused && nact > 1))
     {
         for (int pl = 0; pl < 3; pl++)
         {
