@@ -1487,7 +1487,9 @@ struct hbcu_nlmeans_s
     std::vector<CUtensorMap> maps;        // [slot*3+plane] TMA descriptors of the bordered planes
     std::vector<CUtensorMap> maps3;       // same planes, box height of the v3 8-bit kernel's tile
     std::vector<CUtensorMap> maps3_pre;   // the prefiltered planes (pre_mem), same box
+    std::vector<CUtensorMap> maps3f;      // same planes, box height of nlmeans_v3f_kernel's tile (v3_fused only)
     int v3_nw, v3_rs;                     // v3 kernel shape (warps, rows per warp); v3_nw == 0: off
+    bool v3_fused;                        // range 3 with nf <= 2 runs nlmeans_v3f_kernel (HBCU_NLMEANS_V3_FUSED=0: off)
     float *d_exptable;                    // 3 x 128
     unsigned *d_range_flag;               // sticky: a 16-bit plane held a sample above kFast16Max (see nlmeans_fast16_kernel)
     cudaStream_t s_h2d, s_pad, s_compute, s_d2h;   // s_compute = s_comp[frame index & (n_comp - 1)] of the launch being queued
@@ -1711,6 +1713,66 @@ int launch_v3_pre(FusedParams &fp, cudaStream_t st)
 // (NH = 4) needs 8 warps (its 9-row history does not fit 168 registers).
 struct V3Shape { int nw, rs; };
 constexpr V3Shape kV3Default = { 12, 10 };
+// nlmeans_v3f_kernel keeps no accumulators in shared memory, so its tile can be taller.  12 x 20 (a 240-row tile) was
+// measured against 12 x 30 (H100 80GB HBM3, 700 W power limit): 30-row strips are 3.5 % faster at 4K but 15 % slower
+// at 1080p, whose 360-row tiles leave SMs idle.  168 registers, no spills.
+constexpr V3Shape kV3Fused = { 12, 20 };
+
+template <int NH>
+int launch_v3f(FusedParams &fp, cudaStream_t st)
+{
+    constexpr int NW = kV3Fused.nw, RS = kV3Fused.rs;
+    using L = V3FusedLayout<NW, RS>;
+    // function attributes live in the device's context: one flag per device
+    static bool configured_on[kMaxDevices] = {};
+    int dev_ = 0;
+    HBCU_CHECK(cudaGetDevice(&dev_));
+    bool &configured = configured_on[dev_ & (kMaxDevices - 1)];
+    if (!configured)
+    {
+        HBCU_CHECK(cudaFuncSetAttribute(nlmeans_v3f_kernel<NH, NW, RS>, cudaFuncAttributeMaxDynamicSharedMemorySize, L::kTotal));
+        configured = true;
+    }
+    int total = 0;
+    for (int i = 0; i < fp.nplanes; i++)
+    {
+        fp.first_tile[i] = total;
+        fp.tiles_x[i] = (fp.k[i].w + kTileW - 1) / kTileW;
+        total += fp.tiles_x[i] * ((fp.k[i].h + L::kTH - 1) / L::kTH);
+    }
+    fp.first_tile[fp.nplanes] = total;
+    nlmeans_v3f_kernel<NH, NW, RS><<<total, NW * 32, L::kTotal, st>>>(fp);
+    hbcu::count_launch();
+    return 0;
+}
+
+// nlmeans_v3f_kernel takes a launch whose planes all have range 3 and one or two frames (patch 3 .. 7; the caller has
+// checked that the 8-bit v3 kernel may run them).  More frames keep the accumulating kernel: each further frame would
+// add nine running sums to registers that are full.
+bool v3f_ok(const hbcu_nlmeans_s *h, const KernelParams *kps, const bool *active, int n)
+{
+    if (!h->v3_fused) return false;
+    bool any = false;
+    for (int pl = 0; pl < n; pl++)
+    {
+        if (active != nullptr && !active[pl]) continue;
+        const KernelParams &k = kps[pl];
+        if (k.r_half != 1 || k.nf > 2 || k.n_half < 1 || k.n_half > 3 || k.use_pre) return false;
+        any = true;
+    }
+    return any;
+}
+
+int launch_v3f_nh(FusedParams &fp, cudaStream_t st)
+{
+    switch (fp.k[0].n_half)
+    {
+        case 1: return launch_v3f<1>(fp, st);
+        case 2: return launch_v3f<2>(fp, st);
+        case 3: return launch_v3f<3>(fp, st);
+        default: return 1;
+    }
+}
 
 // rows of one TMA box of the v3 tile: V3Layout::kBoxRows restated for a run-time shape (the kernel's expect-tx byte
 // count and the tensor map must agree)
@@ -1897,8 +1959,9 @@ int launch_plane(hbcu_nlmeans_s *h, const KernelParams &kp, const int *slots, in
             fp.k[0] = kp;
             V3Shape vs;
             const bool v3 = v3_pick(h, kp.n_half, &vs);
-            for (int f = 0; f < kp.nf; f++) fp.maps[0][f] = v3 ? h->maps3[slots[f] * 3 + plane] : tp.maps[f];
-            rc = v3 ? launch_v3_nh(vs.nw, vs.rs, fp, h->s_compute) : launch_fast8_nh(fp, h->s_compute);
+            const bool v3f = v3 && v3f_ok(h, &kp, nullptr, 1);
+            for (int f = 0; f < kp.nf; f++) fp.maps[0][f] = v3f ? h->maps3f[slots[f] * 3 + plane] : v3 ? h->maps3[slots[f] * 3 + plane] : tp.maps[f];
+            rc = v3f ? launch_v3f_nh(fp, h->s_compute) : v3 ? launch_v3_nh(vs.nw, vs.rs, fp, h->s_compute) : launch_fast8_nh(fp, h->s_compute);
         }
         else
             rc = h->bps == 1 ? launch_tiled_nh<uint8_t, kTH8>(tp, h->s_compute) : launch_tiled_nh<uint16_t, kTH16>(tp, h->s_compute);
@@ -2103,14 +2166,15 @@ int run_filter(hbcu_nlmeans_s *h, int64_t index, int navail, int oslot, void *co
         fp.range_flag = nullptr;
         V3Shape vs;
         const bool v3 = v3_pick(h, nh8, &vs);
+        const bool v3f = v3 && v3f_ok(h, kps, active, 3);
         for (int pl = 0; pl < 3; pl++)
         {
             if (!active[pl]) continue;
             fp.k[fp.nplanes] = kps[pl];
-            for (int f = 0; f < kps[pl].nf; f++) fp.maps[fp.nplanes][f] = (v3 ? h->maps3 : h->maps)[slots[pl][f] * 3 + pl];
+            for (int f = 0; f < kps[pl].nf; f++) fp.maps[fp.nplanes][f] = (v3f ? h->maps3f : v3 ? h->maps3 : h->maps)[slots[pl][f] * 3 + pl];
             fp.nplanes++;
         }
-        const int rc8 = v3 ? launch_v3_nh(vs.nw, vs.rs, fp, h->s_compute) : launch_fast8_nh(fp, h->s_compute);
+        const int rc8 = v3f ? launch_v3f_nh(fp, h->s_compute) : v3 ? launch_v3_nh(vs.nw, vs.rs, fp, h->s_compute) : launch_fast8_nh(fp, h->s_compute);
         if (rc8 < 0) { set_error("nlmeans: fused launch failed"); return -1; }
         if (rc8 == 0)
         {
@@ -2219,6 +2283,9 @@ int hbcu_nlmeans_create(hbcu_nlmeans_t **out, const hbcu_nlmeans_config_t *cfg)
         const bool off = h->v3_nw == 0;
         h->v3_nw = off ? 0 : kV3wShape.nw; h->v3_rs = kV3wShape.rs;
     }
+    // range 3 with nf <= 2 on 8-bit planes: the one-march kernel; HBCU_NLMEANS_V3_FUSED=0 keeps the accumulating one (A/B hook)
+    h->v3_fused = h->bps == 1 && h->v3_nw == kV3Default.nw && h->v3_rs == kV3Default.rs;
+    if (const char *e = getenv("HBCU_NLMEANS_V3_FUSED")) h->v3_fused = h->v3_fused && atoi(e) != 0;
     h->ring = cfg->ring_frames > 0 ? cfg->ring_frames : 8;
     h->out_slots = cfg->out_slots > 0 ? cfg->out_slots : 4;
     h->d_exptable = nullptr;
@@ -2298,6 +2365,7 @@ int hbcu_nlmeans_create(hbcu_nlmeans_t **out, const hbcu_nlmeans_config_t *cfg)
     h->maps.resize(h->ring * 3);
     h->maps3.resize(h->ring * 3);
     h->maps3_pre.resize(h->ring * 3);
+    h->maps3f.resize(h->ring * 3);
     for (int s = 0; s < h->ring; s++)
     {
         CK(cudaEventCreateWithFlags(&h->ev_upload[s], cudaEventDisableTiming));
@@ -2330,6 +2398,14 @@ int hbcu_nlmeans_create(hbcu_nlmeans_t **out, const hbcu_nlmeans_config_t *cfg)
                 hbcu::encode_tensor_map_2d(&h->maps3[s * 3 + pl], h->bps, h->ring_mem[s * 3 + pl], (uint64_t)h->g[pl].bw,
                                            (uint64_t)h->g[pl].bh, (uint64_t)h->g[pl].bpitch * h->bps, kTilePW,
                                            v3_box_rows(h->v3_nw, h->v3_rs)) != 0)
+            {
+                hbcu_nlmeans_destroy(h);
+                return -1;
+            }
+            if (h->v3_fused &&
+                hbcu::encode_tensor_map_2d(&h->maps3f[s * 3 + pl], h->bps, h->ring_mem[s * 3 + pl], (uint64_t)h->g[pl].bw,
+                                           (uint64_t)h->g[pl].bh, (uint64_t)h->g[pl].bpitch * h->bps, kTilePW,
+                                           v3_box_rows(kV3Fused.nw, kV3Fused.rs)) != 0)
             {
                 hbcu_nlmeans_destroy(h);
                 return -1;

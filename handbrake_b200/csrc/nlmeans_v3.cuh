@@ -19,7 +19,9 @@
 //     tiles, or the four tiles of the prefilter variant) inside the 227 KB an H100 block can have;
 //   * range 3 without a prefilter (the SYM instantiation): frame 0, the current frame compared with itself, is one march
 //     over four displacements instead of three over eight -- the other four weights are the same floats read one column
-//     left or one row up (V3Sym) -- and it stores the accumulators instead of adding to zero-filled ones.
+//     left or one row up (V3Sym) -- and it stores the accumulators instead of adding to zero-filled ones;
+//   * range 3 with one or two frames (nlmeans_v3f_kernel): frame 1 advances in V3Sym's row step, every pixel is finished
+//     in registers (V3Fused), and without accumulators the tile is twice as tall.
 #pragma once
 
 template <int NW, int RS, int NBUF, int BPS = 1, bool PRE = false>
@@ -547,9 +549,9 @@ struct V3Sym
         for (int k = 0; k < 5; k++) WD[P][k] = weight(VD[k]);
     }
 
-    // output row r in slot K
+    // output row r in slot K: the weight and pixel sums of its nine frame-0 terms
     template <int K>
-    __device__ __forceinline__ void step(int r)
+    __device__ __forceinline__ void terms(int r, float (&ws4)[4], float (&ps4)[4])
     {
         constexpr int P = K % 2, Q = 1 - P;                                      // this row's and the previous row's weights
         constexpr int SM = (K + 1) % 3, S0 = (K + 2) % 3, SP = K % 3;           // pixel rows r-1, r, r+1
@@ -572,7 +574,6 @@ struct V3Sym
 #pragma unroll
         for (int k = 0; k < 5; k++) WA[k] = weight(VA[k]);
         plus_weights<P>();
-        uint32_t accv[8];
 #pragma unroll
         for (int i = 0; i < 4; i++)
         {
@@ -595,8 +596,23 @@ struct V3Sym
             ps = __fadd_rn(ps, __fmul_rn(WC[P][i], pp[i + 1]));
             ws = __fadd_rn(ws, WB[P][i + 1]);                                     // (+1,+1)
             ps = __fadd_rn(ps, __fmul_rn(WB[P][i + 1], pp[i + 2]));
-            accv[v3_acc_slot(i)] = __float_as_uint(ws);
-            accv[4 + v3_acc_slot(i)] = __float_as_uint(ps);
+            ws4[i] = ws;
+            ps4[i] = ps;
+        }
+    }
+
+    // output row r in slot K: its frame-0 sums into the accumulators
+    template <int K>
+    __device__ __forceinline__ void step(int r)
+    {
+        float ws[4], ps[4];
+        terms<K>(r, ws, ps);
+        uint32_t accv[8];
+#pragma unroll
+        for (int i = 0; i < 4; i++)
+        {
+            accv[v3_acc_slot(i)] = __float_as_uint(ws[i]);
+            accv[4 + v3_acc_slot(i)] = __float_as_uint(ps[i]);
         }
         acc.store(r, accv);
     }
@@ -629,7 +645,8 @@ struct V3Sym
         for (int k = 0; k < 4; k++) VC[k] += hC[k];
     }
 
-    __device__ __forceinline__ void run(int rows)
+    // the state of output row -1: slot 0 of the march comes next
+    __device__ __forceinline__ void start()
     {
 #pragma unroll
         for (int k = 0; k < 5; k++) VA[k] = VB[k] = VD[k] = kVBias;
@@ -643,6 +660,11 @@ struct V3Sym
         plus_weights<0>();
         load_pixels<2>(-1);
         load_pixels<0>(0);
+    }
+
+    __device__ __forceinline__ void run(int rows)
+    {
+        start();
 #pragma unroll 1
         for (int r0 = 0; r0 < rows; r0 += 6) rows_from(r0, rows, std::make_integer_sequence<int, 6>{});
         acc.wait_store();
@@ -808,6 +830,259 @@ __global__ void __launch_bounds__(NW * 32, 1) nlmeans_v3_kernel(const __grid_con
             for (int i = 0; i < 4; i++)
                 if (X0 + x + i < p.w) drow[i] = o[i];
         }
+    }
+}
+
+// Range 3 with one or two frames, patch 3 .. 7, no prefilter: the whole filter of a strip in one march (nlmeans_v3f_kernel).
+// Frame 0 is V3Sym's march.  Frame 1 keeps the running sums of its nine displacements in registers and, like V3Sym,
+// recomputes the patch-row sum leaving each of them from the tiles instead of keeping a history; the source words of
+// the entering and the leaving row are the ones V3Sym has just loaded.  The terms of an output pixel are added in
+// registers in the reference's order -- frame 0's nine as V3Sym adds them, then frame 1's, dy = -1, 0, +1 each with
+// dx = -1, 0, +1, one IEEE operation each -- and the pixel is finished and stored at once: no accumulators in shared
+// memory, so the tile is as tall as the registers allow and the strip's one warm-up is spread over twice the rows.
+template <int NH, int NF>
+struct V3Fused
+{
+    using Sym = V3Sym<NH, V3Acc>;
+    static constexpr int PW = kTilePW / 4;           // tile pitch in words
+    static_assert(NF == 1 || NF == 2, "frame count");
+
+    Sym sym;
+    uint32_t V1[3][3][4];                            // frame 1: 2^23-biased running sums of (dy, dx) at pixels x .. x+3
+    float pix1[3][6];                                // frame 1: pixels x-1 .. x+4 of a compare row, slots as Sym::pix
+    const uint32_t *cbase;                           // compare tile word `lane` of output row 0
+    uint8_t *drow;                                   // output row 0 at pixel x
+    int dpitch, xleft;                               // plane pixels from x on
+
+    __device__ __forceinline__ V3Fused(const uint32_t *cur, const uint32_t *cmp, const V3Acc &none, uint32_t lut_lane_addr, float wscale,
+                                       float wbias, double origin_tune, int seg_y0, int lane, uint8_t *drow_, int dpitch_, int xleft_)
+        : sym(cur, none, lut_lane_addr, wscale, wbias, origin_tune, seg_y0, lane), drow(drow_), dpitch(dpitch_), xleft(xleft_)
+    {
+        cbase = cmp + (seg_y0 + kHalo) * PW + lane;
+    }
+
+    // frame-1 patch-row sums of source row t (words a: lane+3 .. lane+5) against compare row t + dy (words q: lane+2 ..
+    // lane+6) for dx = -1, 0, +1: the compare stream one column left, in place and one column right
+    static __device__ __forceinline__ void row_sums1(const uint32_t (&a)[3], const uint32_t (&q)[5], uint32_t (&h)[3][4])
+    {
+        uint32_t D[3][3];
+#pragma unroll
+        for (int w = 0; w < 3; w++)
+        {
+            D[0][w] = __vabsdiffu4(a[w], __funnelshift_r(q[w], q[w + 1], 24));
+            D[1][w] = __vabsdiffu4(a[w], q[w + 1]);
+            D[2][w] = __vabsdiffu4(a[w], __funnelshift_r(q[w + 1], q[w + 2], 8));
+        }
+#pragma unroll
+        for (int dx = 0; dx < 3; dx++) Sym::template windows<0>(D[dx], h[dx], std::make_integer_sequence<int, 4>{});
+    }
+
+    __device__ __forceinline__ void cmp_words(int row, uint32_t (&q)[5]) const
+    {
+#pragma unroll
+        for (int k = 0; k < 5; k++) q[k] = cbase[row * PW + 2 + k];
+    }
+
+    template <int S>
+    __device__ __forceinline__ void load_pixels1(int row)
+    {
+        const uint32_t *w = cbase + row * PW + 3;
+        const uint32_t w0 = w[0], w1 = w[1], w2 = w[2];
+        pix1[S][0] = __fadd_rn(byte_as_biased_float(w0, 3), -8388608.0f);
+#pragma unroll
+        for (int i = 0; i < 4; i++) pix1[S][1 + i] = __fadd_rn(byte_as_biased_float(w1, i), -8388608.0f);
+        pix1[S][5] = __fadd_rn(byte_as_biased_float(w2, 0), -8388608.0f);
+    }
+
+    // frame 1 moves from output row r-1 to r: patch rows r+NH (source words in Sym::qi[Q]) enter, r-NH-1 (Sym::qo[Q]) leave
+    template <int Q>
+    __device__ __forceinline__ void advance1(int r)
+    {
+        const uint32_t ai[3] = { sym.qi[Q][1], sym.qi[Q][2], sym.qi[Q][3] };
+        const uint32_t ao[3] = { sym.qo[Q][1], sym.qo[Q][2], sym.qo[Q][3] };
+#pragma unroll
+        for (int dy = 0; dy < 3; dy++)
+        {
+            uint32_t q[5], hi[3][4], ho[3][4];
+            cmp_words(r + NH + dy - 1, q);
+            row_sums1(ai, q, hi);
+            cmp_words(r - NH - 2 + dy, q);
+            row_sums1(ao, q, ho);
+#pragma unroll
+            for (int dx = 0; dx < 3; dx++)
+#pragma unroll
+                for (int i = 0; i < 4; i++) V1[dy][dx][i] = V1[dy][dx][i] + hi[dx][i] - ho[dx][i];
+        }
+    }
+
+    // output row r in slot K (Sym's slots)
+    template <int K>
+    __device__ __forceinline__ void step(int r)
+    {
+        float ws[4], ps[4];
+        sym.template terms<K>(r, ws, ps);
+        if constexpr (NF == 2)
+        {
+            constexpr int Q = 1 - K % 2;
+            constexpr int S[3] = { (K + 1) % 3, (K + 2) % 3, K % 3 };            // compare pixel rows r-1, r, r+1
+            advance1<Q>(r);
+            load_pixels1<S[2]>(r + 1);
+#pragma unroll
+            for (int dy = 0; dy < 3; dy++)
+#pragma unroll
+                for (int dx = 0; dx < 3; dx++)
+#pragma unroll
+                    for (int i = 0; i < 4; i++)
+                    {
+                        const float w = sym.weight(V1[dy][dx][i]);
+                        ws[i] = __fadd_rn(ws[i], w);
+                        ps[i] = __fadd_rn(ps[i], __fmul_rn(w, pix1[S[dy]][i + dx]));
+                    }
+        }
+        const uint32_t cwd = sym.base[r * PW + kHaloX / 4];
+        uint8_t o[4];
+#pragma unroll
+        for (int i = 0; i < 4; i++) o[i] = finish_pixel<uint8_t>(ws[i], ps[i], (uint8_t)((cwd >> (8 * i)) & 0xffu));
+        uint8_t *d = drow + (size_t)r * dpitch;
+        if (xleft >= 4)
+            *reinterpret_cast<uchar4 *>(d) = make_uchar4(o[0], o[1], o[2], o[3]);
+        else
+        {
+#pragma unroll
+            for (int i = 0; i < 4; i++)
+                if (i < xleft) d[i] = o[i];
+        }
+    }
+
+    template <int... Ms>
+    __device__ __forceinline__ void rows_from(int r0, int rows, std::integer_sequence<int, Ms...>)
+    {
+        ((r0 + Ms < rows ? step<(Ms + 1) % 6>(r0 + Ms) : (void)0), ...);
+    }
+
+    __device__ __forceinline__ void run(int rows)
+    {
+        sym.start();
+        if constexpr (NF == 2)
+        {
+            // the state of output row -1, as Sym's: the sums of patch rows -NH-1 .. NH-1, compare pixel rows -1 and 0
+#pragma unroll
+            for (int dy = 0; dy < 3; dy++)
+#pragma unroll
+                for (int dx = 0; dx < 3; dx++)
+#pragma unroll
+                    for (int i = 0; i < 4; i++) V1[dy][dx][i] = kVBias;
+#pragma unroll 1
+            for (int t = -NH - 1; t < NH; t++)
+            {
+                const uint32_t *s = sym.base + t * PW + 3;
+                const uint32_t a[3] = { s[0], s[1], s[2] };
+#pragma unroll
+                for (int dy = 0; dy < 3; dy++)
+                {
+                    uint32_t q[5], h[3][4];
+                    cmp_words(t + dy - 1, q);
+                    row_sums1(a, q, h);
+#pragma unroll
+                    for (int dx = 0; dx < 3; dx++)
+#pragma unroll
+                        for (int i = 0; i < 4; i++) V1[dy][dx][i] += h[dx][i];
+                }
+            }
+            load_pixels1<2>(-1);
+            load_pixels1<0>(0);
+        }
+#pragma unroll 1
+        for (int r0 = 0; r0 < rows; r0 += 6) rows_from(r0, rows, std::make_integer_sequence<int, 6>{});
+    }
+};
+
+// Shared memory of nlmeans_v3f_kernel: the current tile, one compare tile, the weight table
+template <int NW, int RS>
+struct V3FusedLayout
+{
+    static constexpr int kTH        = NW * RS;
+    static constexpr int kLoads     = kTH + 2 * kHalo > 256 ? 2 : 1;                     // a TMA box has at most 256 rows
+    static constexpr int kBoxRows   = ((kTH + 2 * kHalo + kLoads - 1) / kLoads + 3) / 4 * 4;
+    static constexpr int kTileBytes = kBoxRows * kLoads * kTilePW;
+    static constexpr int kLutBytes  = kLutEntries * 32 * (int)sizeof(float);
+    static constexpr int kOffCur    = 0;
+    static constexpr int kOffCmp    = kOffCur + kTileBytes;
+    static constexpr int kOffLut    = kOffCmp + kTileBytes;
+    static constexpr int kOffBar    = kOffLut + kLutBytes;                               // 2 mbarriers
+    static constexpr int kTotal     = kOffBar + 64;
+    static_assert(kBoxRows <= 256, "TMA box rows");
+    static_assert((kBoxRows * kTilePW) % 128 == 0, "TMA destination must stay 128-byte aligned");
+    static_assert(kTotal <= 227 * 1024, "shared memory");
+};
+
+// Every plane of the launch at range 3 with nf <= 2, patch 3 .. 7 and no prefilter (launch_v3f): V3Fused per strip.
+template <int NH, int NW, int RS>
+__global__ void __launch_bounds__(NW * 32, 1) nlmeans_v3f_kernel(const __grid_constant__ FusedParams fp)
+{
+    static_assert(NH >= 1 && NH <= 3, "patch 3 .. 7");
+    constexpr int kThreads = NW * 32;
+    using L = V3FusedLayout<NW, RS>;
+    int pl = 0;
+    while (pl + 1 < fp.nplanes && (int)blockIdx.x >= fp.first_tile[pl + 1]) pl++;
+    const KernelParams &p = fp.k[pl];
+    const CUtensorMap *maps = fp.maps[pl];
+    const int tile = (int)blockIdx.x - fp.first_tile[pl];
+    extern __shared__ __align__(128) uint8_t smem[];
+    uint8_t *cur  = smem + L::kOffCur;
+    uint8_t *cmp  = smem + L::kOffCmp;
+    float *lut    = reinterpret_cast<float *>(smem + L::kOffLut);
+    uint64_t *bar = reinterpret_cast<uint64_t *>(smem + L::kOffBar);           // [0] current tile, [1] compare tile
+
+    const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
+    const int X0 = (tile % fp.tiles_x[pl]) * kTileW, Y0 = (tile / fp.tiles_x[pl]) * L::kTH;
+    const int gx = X0 + kBorder - kHaloX, gy = Y0 + kBorder - kHalo;
+
+    if (tid == 0)
+    {
+        mbar_init(bar, 1);
+        mbar_init(bar + 1, 1);
+        asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
+    }
+    __syncthreads();
+    if (tid == 0)
+    {
+        mbar_expect_tx(bar, L::kTileBytes);
+        for (int l = 0; l < L::kLoads; l++) tma_load_2d(cur + l * L::kBoxRows * kTilePW, &maps[0], gx, gy + l * L::kBoxRows, bar);
+        if (p.nf > 1)
+        {
+            mbar_expect_tx(bar + 1, L::kTileBytes);
+            for (int l = 0; l < L::kLoads; l++) tma_load_2d(cmp + l * L::kBoxRows * kTilePW, &maps[1], gx, gy + l * L::kBoxRows, bar + 1);
+        }
+    }
+    for (int i = tid; i < kLutEntries * 32; i += kThreads)
+    {
+        const int e = i >> 5;
+        lut[i] = e < HBCU_NLMEANS_EXPSIZE ? p.exptable[e] : 0.f;
+    }
+
+    const int seg_y0 = warp * RS;
+    int rows = p.h - (Y0 + seg_y0);                                     // rows of this warp's strip inside the plane
+    rows = rows < 0 ? 0 : (rows > RS ? RS : rows);
+    mbar_wait(bar, 0);
+    __syncthreads();
+    if (rows == 0) return;
+
+    const float wscale = p.wfact * 0.0078125f;                         // wfact / 128, exact
+    const float wbias  = -8388608.0f * wscale;                         // exact (power-of-two scaling)
+    // shared address of this lane's copy of table entry 0, pre-biased by -(0x47800000 << 7)
+    const uint32_t lut_lane_addr = smem_u32(lut) + (uint32_t)lane * 4u - (0x47800000u << 7);
+    const uint32_t *cw = reinterpret_cast<const uint32_t *>(cur);
+    const uint32_t *bw = reinterpret_cast<const uint32_t *>(cmp);
+    const V3Acc none = { nullptr, nullptr };
+    uint8_t *drow = reinterpret_cast<uint8_t *>(p.dst) + (size_t)(Y0 + seg_y0) * p.dpitch + X0 + lane * 4;
+    const int xleft = p.w - (X0 + lane * 4);
+    if (p.nf == 1)
+        V3Fused<NH, 1>(cw, bw, none, lut_lane_addr, wscale, wbias, p.origin_tune, seg_y0, lane, drow, p.dpitch, xleft).run(rows);
+    else
+    {
+        mbar_wait(bar + 1, 0);
+        V3Fused<NH, 2>(cw, bw, none, lut_lane_addr, wscale, wbias, p.origin_tune, seg_y0, lane, drow, p.dpitch, xleft).run(rows);
     }
 }
 
