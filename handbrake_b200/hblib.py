@@ -23,6 +23,22 @@ class HarnessIO(C.Structure):
     ]
 
 
+class HarnessOverlay(C.Structure):
+    _fields_ = [("frame", C.c_int), ("x", C.c_int), ("y", C.c_int), ("width", C.c_int), ("height", C.c_int),
+                ("yuva", C.c_void_p)]
+
+
+class HarnessBlend(C.Structure):
+    _fields_ = [("blend", C.c_void_p), ("overlay_pix_fmt", C.c_int), ("chroma_location", C.c_int),
+                ("n_overlays", C.c_int), ("overlays", C.c_void_p), ("n_changed", C.c_int), ("changed", C.c_void_p),
+                ("guard_x", C.c_int), ("guard_y", C.c_int),
+                ("guard_damaged", C.c_int), ("same_buffer", C.c_int), ("frames", C.c_int)]
+
+
+# the render_sub stand-in of the harness (hb_harness.h): put it in a chain with run_blend()
+RENDER_SUB = "hb_filter_render_sub_harness"
+
+
 class FilterResult:
     def __init__(self):
         self.frames = None
@@ -54,6 +70,32 @@ class FilterLib:
         """address of the exported hb_filter_object_t `name` (e.g. 'hb_filter_nlmeans')"""
         return C.addressof(C.c_char.in_dll(self.lib, name))
 
+    def run_blend(self, blend, overlays, overlay_pix_fmt, filters, settings, frames, pix_fmt, width, height,
+                  chroma_location=2, changed=None, guard=(0, 0), **kw):
+        """run a chain holding RENDER_SUB, which burns `overlays` into the frames through the exported blend object
+        `blend` ('hb_blend', 'hb_blend_cuda').  overlays: (frame, x, y, width, height, yuva) in list order, yuva the
+        overlay's planes Y, Cb, Cr, A packed at their widths (uint8); changed: per-frame flags (default 1);
+        guard: (columns, rows) of spare samples around host frames while the blend object works on them.
+        Returns (FilterResult, dict(guard_damaged, same_buffer, frames))."""
+        keep = [np.ascontiguousarray(o[5], dtype=np.uint8) for o in overlays]
+        arr = (HarnessOverlay * max(1, len(overlays)))()
+        for i, (o, data) in enumerate(zip(overlays, keep)):
+            arr[i] = HarnessOverlay(int(o[0]), int(o[1]), int(o[2]), int(o[3]), int(o[4]), data.ctypes.data)
+        ch = np.ascontiguousarray(changed if changed is not None else [], dtype=np.int32)
+        cfg = HarnessBlend()
+        cfg.blend = self.filter_object(blend)
+        cfg.overlay_pix_fmt, cfg.chroma_location = int(overlay_pix_fmt), int(chroma_location)
+        cfg.n_overlays, cfg.overlays = len(overlays), C.addressof(arr)
+        cfg.n_changed, cfg.changed = len(ch), ch.ctypes.data
+        cfg.guard_x, cfg.guard_y = int(guard[0]), int(guard[1])
+        self.lib.hb_harness_set_blend.argtypes = [C.c_void_p]
+        self.lib.hb_harness_set_blend(C.addressof(cfg))
+        try:
+            r = self.run(filters, settings, frames, pix_fmt, width, height, **kw)
+        finally:
+            self.lib.hb_harness_set_blend(None)
+        return r, dict(guard_damaged=cfg.guard_damaged, same_buffer=cfg.same_buffer, frames=cfg.frames)
+
     def buffers_alive(self):
         return int(self.lib.hb_shim_buffers_alive())
 
@@ -68,7 +110,7 @@ class FilterLib:
             filters, settings = [filters], [settings]
         frames = np.ascontiguousarray(frames, dtype=np.uint8)
         n_in = frames.shape[0]
-        fb = synth.frame_bytes(pix_fmt, width, height)
+        fb = int(self.lib.hb_harness_frame_bytes(pix_fmt, width, height))     # any format the shim knows
         assert frames.shape[1] == fb, (frames.shape, fb)
         cap = max_out if max_out is not None else (n_in * 2 * out_scale + 8)
         out = np.zeros((cap, fb), dtype=np.uint8)

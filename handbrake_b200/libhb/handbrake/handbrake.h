@@ -79,9 +79,26 @@ enum AVPixelFormat
     /* FFmpeg's hardware pixel format for CUDA frames.  libhb signals hardware frames through
      * hb_filter_init_t.hw_pix_fmt / job->hw_pix_fmt (nvenc_common.c:329-336); the value is only ever compared */
     AV_PIX_FMT_CUDA        = 117,
+    /* the overlay formats of libhb's subtitle renderer (rendersub.c): planar YUV with an 8-bit alpha plane */
+    AV_PIX_FMT_YUVA420P    = 33,
+    AV_PIX_FMT_YUVA422P    = 78,
+    AV_PIX_FMT_YUVA444P    = 79,
 };
 #define AV_PIX_FMT_YUV420P10 AV_PIX_FMT_YUV420P10LE
 #define AV_PIX_FMT_YUV420P12 AV_PIX_FMT_YUV420P12LE
+
+/* FFmpeg's enum AVChromaLocation (libavutil/pixfmt.h) */
+enum AVChromaLocation
+{
+    AVCHROMA_LOC_UNSPECIFIED = 0,
+    AVCHROMA_LOC_LEFT        = 1,
+    AVCHROMA_LOC_CENTER      = 2,
+    AVCHROMA_LOC_TOPLEFT     = 3,
+    AVCHROMA_LOC_TOP         = 4,
+    AVCHROMA_LOC_BOTTOMLEFT  = 5,
+    AVCHROMA_LOC_BOTTOM      = 6,
+    AVCHROMA_LOC_NB
+};
 
 typedef struct AVComponentDescriptor
 {
@@ -104,6 +121,8 @@ typedef struct AVPixFmtDescriptor
 
 const AVPixFmtDescriptor *av_pix_fmt_desc_get(int pix_fmt);
 int av_image_get_linesize(int pix_fmt, int width, int plane);
+/* number of distinct planes of the format (libavutil/pixdesc.c), < 0 for an unknown format */
+int av_pix_fmt_count_planes(int pix_fmt);
 
 typedef struct AVRational { int num; int den; } AVRational;
 typedef struct AVChannelLayout { int order; int nb_channels; uint64_t mask; void *opaque; } AVChannelLayout;
@@ -219,6 +238,9 @@ void          hb_buffer_close(hb_buffer_t **);
 hb_buffer_t * hb_buffer_dup(const hb_buffer_t *src);
 hb_buffer_t * hb_buffer_shallow_dup(const hb_buffer_t *src);
 int           hb_buffer_copy(hb_buffer_t *dst, const hb_buffer_t *src);
+/* fifo.c:624-639: may the holder write into the buffer's planes?  Host buffers (STANDARD, HBCU_PINNED) yes; an
+ * HBCU_DEVICE buffer never -- a device frame is written once, by its producer */
+int           hb_buffer_is_writable(const hb_buffer_t *buf);
 void          hb_buffer_copy_props(hb_buffer_t *dst, const hb_buffer_t *src);
 
 /* allocator hook: lets the CUDA filters make every frame buffer page-locked
@@ -457,6 +479,24 @@ extern hb_filter_object_t hb_filter_decomb;
 #endif
 static inline void *av_malloc(size_t size) { void *p = NULL; if (posix_memalign(&p, 64, size ? size : 1) != 0) return NULL; return p; }
 static inline void av_freep(void *arg) { void **pp = (void **)arg; free(*pp); *pp = NULL; }
+
+/* ---- blend objects: composite a list of YUVA overlays onto a frame (handbrake/common.h:1813-1826) ---- */
+typedef struct hb_blend_object_s  hb_blend_object_t;
+typedef struct hb_blend_private_s hb_blend_private_t;   /* handbrake/hbtypes.h:46-47 */
+struct hb_blend_object_s
+{
+    char                * name;
+    int                (* init)  (hb_blend_object_t *, int in_width, int in_height, int in_pix_fmt, int in_chroma_location,
+                                  int in_color_range, int overlay_pix_fmt);
+    hb_buffer_t *      (* work)  (hb_blend_object_t *, hb_buffer_t *, hb_buffer_list_t *, int changed);
+    void               (* close) (hb_blend_object_t *);
+    hb_blend_private_t  * private_data;
+};
+extern hb_blend_object_t hb_blend;
+
+/* common.c:7054-7091: the per-position weights [0][x] / [1][y] of the luma samples that make up one chroma sample,
+ * from the format's subsampling and the chroma location */
+void hb_compute_chroma_smoothing_coefficient(uint32_t chroma_coeffs[2][4], int pix_fmt, int chroma_location);
 
 extern hb_filter_object_t hb_filter_denoise;
 extern hb_filter_object_t hb_filter_detelecine;

@@ -235,3 +235,218 @@ int hb_harness_run(hb_filter_object_t *proto, const char *settings, hb_harness_i
     const char *sets[1] = { settings };
     return hb_harness_run_chain(1, protos, sets, io);
 }
+
+/* ------------------------------------------------------------------ */
+/* render_sub stand-in                                                  */
+/* ------------------------------------------------------------------ */
+#define GUARD_BYTE 0x5a
+
+static hb_harness_blend_t *g_blend_cfg = NULL;
+
+void hb_harness_set_blend(hb_harness_blend_t *cfg) { g_blend_cfg = cfg; }
+
+struct hb_filter_private_s
+{
+    hb_harness_blend_t *cfg;
+    hb_blend_object_t   blend;        /* this instance's copy of the object (its private_data is per instance) */
+    int                 frame, next_overlay;
+};
+
+static int  render_sub_harness_init(hb_filter_object_t *filter, hb_filter_init_t *init);
+static int  render_sub_harness_work(hb_filter_object_t *filter, hb_buffer_t **buf_in, hb_buffer_t **buf_out);
+static void render_sub_harness_close(hb_filter_object_t *filter);
+
+hb_filter_object_t hb_filter_render_sub_harness =
+{
+    .id            = HB_FILTER_RENDER_SUB,
+    .enforce_order = 1,
+    .name          = "Subtitle burn-in (test stand-in for render_sub)",
+    .short_name    = "render_sub_harness",
+    .init          = render_sub_harness_init,
+    .work          = render_sub_harness_work,
+    .close         = render_sub_harness_close,
+};
+
+static int render_sub_harness_init(hb_filter_object_t *filter, hb_filter_init_t *init)
+{
+    hb_harness_blend_t *cfg = g_blend_cfg;
+    if (cfg == NULL || cfg->blend == NULL)
+    {
+        hb_error("render_sub_harness: no blend schedule set");
+        return -1;
+    }
+    hb_filter_private_t *pv = calloc(1, sizeof(*pv));
+    if (pv == NULL) return -1;
+    pv->cfg = cfg;
+    pv->blend = *cfg->blend;
+    pv->blend.private_data = NULL;
+    cfg->guard_damaged = cfg->same_buffer = cfg->frames = 0;
+    /* rendersub.c:1129-1160 (hb_blend_init): the frame's geometry, format and chroma location, the overlay format */
+    if (pv->blend.init(&pv->blend, init->geometry.width, init->geometry.height, init->pix_fmt, cfg->chroma_location,
+                       init->color_range, cfg->overlay_pix_fmt) != 0)
+    {
+        if (pv->blend.close) pv->blend.close(&pv->blend);
+        free(pv);
+        return -1;
+    }
+    filter->private_data = pv;
+    return 0;
+}
+
+static void render_sub_harness_close(hb_filter_object_t *filter)
+{
+    hb_filter_private_t *pv = filter->private_data;
+    if (pv == NULL) return;
+    pv->blend.close(&pv->blend);
+    free(pv);
+    filter->private_data = NULL;
+}
+
+static int plane_bps(const hb_buffer_t *b)
+{
+    const AVPixFmtDescriptor *d = av_pix_fmt_desc_get(b->f.fmt);
+    return d->comp[0].depth > 8 ? 2 : 1;
+}
+
+/* a host frame with guard_x spare samples and guard_y spare rows around every plane, filled with GUARD_BYTE: writes
+ * outside the picture land in memory the frame owns and can be found afterwards */
+static hb_buffer_t *guarded_copy(const hb_buffer_t *in, int gx, int gy)
+{
+    const int bps = plane_bps(in);
+    int stride[3], size = 0;
+    for (int p = 0; p < 3; p++)
+    {
+        stride[p] = HB_ALIGN((in->plane[p].width + 2 * gx) * bps, 64);
+        size += stride[p] * (in->plane[p].height + 2 * gy);
+    }
+    hb_buffer_t *b = hb_buffer_init(size);
+    if (b == NULL) return NULL;
+    memset(b->data, GUARD_BYTE, size);
+    b->f = in->f;
+    hb_buffer_copy_props(b, in);
+    uint8_t *base = b->data;
+    for (int p = 0; p < 3; p++)
+    {
+        b->plane[p] = in->plane[p];
+        b->plane[p].stride = stride[p];
+        b->plane[p].data = base + (size_t)gy * stride[p] + (size_t)gx * bps;
+        b->plane[p].size = stride[p] * in->plane[p].height;
+        for (int y = 0; y < in->plane[p].height; y++)
+            memcpy(b->plane[p].data + (size_t)y * stride[p], in->plane[p].data + (size_t)y * in->plane[p].stride,
+                   (size_t)in->plane[p].width * bps);
+        base += (size_t)stride[p] * (in->plane[p].height + 2 * gy);
+    }
+    return b;
+}
+
+/* every byte of the guarded allocation outside the pictures still GUARD_BYTE? */
+static int guard_intact(const hb_buffer_t *b, int gx, int gy)
+{
+    const int bps = plane_bps(b);
+    for (int p = 0; p < 3; p++)
+    {
+        const int stride = b->plane[p].stride, w = b->plane[p].width * bps, h = b->plane[p].height;
+        const uint8_t *row0 = b->plane[p].data - (size_t)gy * stride - (size_t)gx * bps;
+        for (int y = 0; y < h + 2 * gy; y++)
+        {
+            const uint8_t *r = row0 + (size_t)y * stride;
+            const int inside = y >= gy && y < gy + h;
+            for (int x = 0; x < stride; x++)
+                if ((!inside || x < gx * bps || x >= gx * bps + w) && r[x] != GUARD_BYTE) return 0;
+        }
+    }
+    return 1;
+}
+
+static hb_buffer_t *unguarded_copy(const hb_buffer_t *g)
+{
+    hb_buffer_t *b = hb_frame_buffer_init(g->f.fmt, g->f.width, g->f.height);
+    if (b == NULL) return NULL;
+    const hb_buffer_t tmp = *b;
+    b->f = g->f;
+    b->f.max_plane = tmp.f.max_plane;
+    hb_buffer_copy_props(b, g);
+    const int bps = plane_bps(g);
+    for (int p = 0; p < 3; p++)
+        for (int y = 0; y < b->plane[p].height; y++)
+            memcpy(b->plane[p].data + (size_t)y * b->plane[p].stride, g->plane[p].data + (size_t)y * g->plane[p].stride,
+                   (size_t)b->plane[p].width * bps);
+    return b;
+}
+
+/* this frame's overlays as rendersub hands them over: YUVA buffers at f.x / f.y, linked in list order */
+static int build_overlays(hb_filter_private_t *pv, hb_buffer_list_t *list)
+{
+    const hb_harness_blend_t *cfg = pv->cfg;
+    hb_buffer_list_clear(list);
+    while (pv->next_overlay < cfg->n_overlays && cfg->overlays[pv->next_overlay].frame < pv->frame) pv->next_overlay++;
+    for (; pv->next_overlay < cfg->n_overlays && cfg->overlays[pv->next_overlay].frame == pv->frame; pv->next_overlay++)
+    {
+        const hb_harness_overlay_t *o = &cfg->overlays[pv->next_overlay];
+        hb_buffer_t *b = hb_frame_buffer_init(cfg->overlay_pix_fmt, o->width, o->height);
+        if (b == NULL) return -1;
+        b->f.x = o->x;
+        b->f.y = o->y;
+        const uint8_t *src = o->yuva;
+        for (int p = 0; p < 4; p++)
+            for (int y = 0; y < b->plane[p].height; y++)
+            {
+                memcpy(b->plane[p].data + (size_t)y * b->plane[p].stride, src, b->plane[p].width);
+                src += b->plane[p].width;
+            }
+        hb_buffer_list_append(list, b);
+    }
+    return 0;
+}
+
+static int render_sub_harness_work(hb_filter_object_t *filter, hb_buffer_t **buf_in, hb_buffer_t **buf_out)
+{
+    hb_filter_private_t *pv = filter->private_data;
+    hb_harness_blend_t *cfg = pv->cfg;
+    hb_buffer_t *in = *buf_in;
+    *buf_in = NULL;
+    if (in->s.flags & HB_BUF_FLAG_EOF)
+    {
+        *buf_out = in;
+        return HB_FILTER_DONE;
+    }
+    hb_buffer_list_t overlays;
+    if (build_overlays(pv, &overlays) != 0)
+    {
+        hb_buffer_list_close(&overlays);
+        hb_buffer_close(&in);
+        return HB_FILTER_FAILED;
+    }
+    const int changed = pv->frame < cfg->n_changed ? cfg->changed[pv->frame] : 1;
+    pv->frame++;
+    cfg->frames++;
+
+    const int guarded = (cfg->guard_x > 0 || cfg->guard_y > 0) && in->storage_type != HBCU_DEVICE;
+    if (guarded)
+    {
+        hb_buffer_t *g = guarded_copy(in, cfg->guard_x, cfg->guard_y);
+        hb_buffer_close(&in);
+        if (g == NULL)
+        {
+            hb_buffer_list_close(&overlays);
+            return HB_FILTER_FAILED;
+        }
+        in = g;
+    }
+    const hb_buffer_t *given = in;
+    hb_buffer_t *out = pv->blend.work(&pv->blend, in, &overlays, changed);
+    hb_buffer_list_close(&overlays);            /* rendersub drops its overlays as soon as work() returns */
+    if (out == NULL)
+        return HB_FILTER_FAILED;
+    if (out == given) cfg->same_buffer++;
+    if (guarded)
+    {
+        if (!guard_intact(out, cfg->guard_x, cfg->guard_y)) cfg->guard_damaged++;
+        hb_buffer_t *plain = unguarded_copy(out);
+        hb_buffer_close(&out);
+        if (plain == NULL) return HB_FILTER_FAILED;
+        out = plain;
+    }
+    *buf_out = out;
+    return HB_FILTER_OK;
+}

@@ -36,6 +36,36 @@ int hb_harness_run(hb_filter_object_t *proto, const char *settings, hb_harness_i
 int hb_harness_run_chain(int n_filters, hb_filter_object_t *const *protos,
                          const char *const *settings, hb_harness_io_t *io);
 
+/* ---- a stand-in for libhb's render_sub filter (rendersub.c): burns a per-frame schedule of overlays into the frames
+ * through a blend object (hb_blend, hb_blend_cuda ...), calling its init / work / close the way rendersub does ---- */
+typedef struct hb_harness_overlay_s
+{
+    int            frame;             /* index of the input frame it is shown on */
+    int            x, y, width, height;
+    const uint8_t *yuva;              /* the overlay's planes Y, Cb, Cr, A back to back, rows packed at the plane widths */
+} hb_harness_overlay_t;
+
+typedef struct hb_harness_blend_s
+{
+    /* input */
+    hb_blend_object_t          *blend;
+    int                         overlay_pix_fmt, chroma_location;
+    int                         n_overlays;
+    const hb_harness_overlay_t *overlays;     /* ordered by frame; within a frame, list order */
+    int                         n_changed;
+    const int                  *changed;      /* per frame; frames past n_changed pass changed = 1 */
+    int                         guard_x, guard_y;   /* > 0: host frames get this many spare samples / rows on every side
+                                                     * around the picture while the blend object works on them */
+    /* output */
+    int                         guard_damaged;  /* frames where a sample outside the picture was written */
+    int                         same_buffer;    /* frames whose work() handed back the buffer it was given */
+    int                         frames;
+} hb_harness_blend_t;
+
+/* the schedule the next chains' hb_filter_render_sub_harness instances use (the caller keeps it alive) */
+void hb_harness_set_blend(hb_harness_blend_t *cfg);
+extern hb_filter_object_t hb_filter_render_sub_harness;
+
 #ifdef __cplusplus
 }
 #endif

@@ -34,6 +34,11 @@ static const AVPixFmtDescriptor desc_yuv422p10  = DESC("yuv422p10le", 1, 0, 10, 
 static const AVPixFmtDescriptor desc_yuv444p10  = DESC("yuv444p10le", 0, 0, 10, 3);
 static const AVPixFmtDescriptor desc_yuv420p12  = DESC("yuv420p12le", 1, 1, 12, 3);
 static const AVPixFmtDescriptor desc_yuv420p16  = DESC("yuv420p16le", 1, 1, 16, 3);
+#define DESC_A(nm, cw, ch) \
+    { nm, 4, cw, ch, 0, { {0, 0, 0, 0, 8}, {1, 0, 0, 0, 8}, {2, 0, 0, 0, 8}, {3, 0, 0, 0, 8} } }
+static const AVPixFmtDescriptor desc_yuva420p   = DESC_A("yuva420p", 1, 1);
+static const AVPixFmtDescriptor desc_yuva422p   = DESC_A("yuva422p", 1, 0);
+static const AVPixFmtDescriptor desc_yuva444p   = DESC_A("yuva444p", 0, 0);
 
 const AVPixFmtDescriptor *av_pix_fmt_desc_get(int pix_fmt)
 {
@@ -48,7 +53,44 @@ const AVPixFmtDescriptor *av_pix_fmt_desc_get(int pix_fmt)
         case AV_PIX_FMT_YUV444P10LE: return &desc_yuv444p10;
         case AV_PIX_FMT_YUV420P12LE: return &desc_yuv420p12;
         case AV_PIX_FMT_YUV420P16LE: return &desc_yuv420p16;
+        case AV_PIX_FMT_YUVA420P:    return &desc_yuva420p;
+        case AV_PIX_FMT_YUVA422P:    return &desc_yuva422p;
+        case AV_PIX_FMT_YUVA444P:    return &desc_yuva444p;
         default:                     return NULL;
+    }
+}
+
+int av_pix_fmt_count_planes(int pix_fmt)
+{
+    const AVPixFmtDescriptor *d = av_pix_fmt_desc_get(pix_fmt);
+    if (d == NULL) return -1;
+    int seen[4] = {0, 0, 0, 0}, n = 0;
+    for (int c = 0; c < d->nb_components; c++)
+        if (!seen[d->comp[c].plane]++) n++;
+    return n;
+}
+
+/* Restatement of common.c:7054-7091.  Weak: the reference build (oracle/Makefile) links the reference's own definition
+ * next to this file, and that one must win there. */
+__attribute__((weak)) void hb_compute_chroma_smoothing_coefficient(uint32_t chroma_coeffs[2][4], int pix_fmt, int chroma_location)
+{
+    const AVPixFmtDescriptor *desc = av_pix_fmt_desc_get(pix_fmt);
+    const int sw = desc->log2_chroma_w, sh = desc->log2_chroma_h;
+    /* the offset into the 1 3 9 27 9 3 1 kernel of the first luma sample of a chroma group: centred by default, one
+     * sample further for every side the chroma location pins the sample to */
+    int wx = 4 - (1 << sw), wy = 4 - (1 << sh);
+    const int left = chroma_location == AVCHROMA_LOC_TOPLEFT || chroma_location == AVCHROMA_LOC_LEFT ||
+                     chroma_location == AVCHROMA_LOC_BOTTOMLEFT;
+    const int vert = chroma_location == AVCHROMA_LOC_TOPLEFT || chroma_location == AVCHROMA_LOC_TOP ||
+                     chroma_location == AVCHROMA_LOC_BOTTOMLEFT || chroma_location == AVCHROMA_LOC_BOTTOM;
+    if (left) wx += (1 << sw) - 1;
+    if (vert) wy += (1 << sh) - 1;
+    static const uint32_t base[7] = {1, 3, 9, 27, 9, 3, 1};
+    /* an even offset averages two neighbouring kernel taps (the sample sits between them) */
+    for (int i = 0; i < 4; i++)
+    {
+        chroma_coeffs[0][i] = (base[i + wx] + base[i + wx + ((wx & 1) == 0)]) >> 1;
+        chroma_coeffs[1][i] = (base[i + wy] + base[i + wy + ((wy & 1) == 0)]) >> 1;
     }
 }
 
@@ -383,6 +425,11 @@ hb_buffer_t *hb_buffer_dup(const hb_buffer_t *src)
     if (buf->s.type == FRAME_BUF) hb_buffer_init_planes(buf);
     if (src->size > 0) memcpy(buf->data, src->data, src->size);
     return buf;
+}
+
+int hb_buffer_is_writable(const hb_buffer_t *buf)
+{
+    return buf->storage_type == STANDARD || buf->storage_type == HBCU_PINNED;
 }
 
 /* STANDARD buffers have no refcount in libhb either: shallow dup == dup (fifo.c:718-721) */

@@ -455,6 +455,52 @@ int  hbcu_detelecine_download_frame(hbcu_detelecine_t *h, int picture, hbcu_fram
 int  hbcu_detelecine_mark(hbcu_detelecine_t *h, int which);
 int  hbcu_detelecine_elapsed_ms(hbcu_detelecine_t *h, float *ms);
 
+/* ------------------------------------------------------------------------- */
+/* blend        replaces the overlay compositing of libhb/blend.c (blend8on8,   */
+/*              blend8on1x, blend_subsample_8on8, blend_subsample_8on1x):        */
+/*              burned-in subtitles (rendersub.c) on planar YUV frames           */
+/* ------------------------------------------------------------------------- */
+/* One handle per frame geometry.  Overlays are 8-bit YUVA with the frame's chroma subsampling (the plain path of
+ * blend.c) or YUVA 4:4:4 on a subsampled frame (the subsample path: every chroma sample takes the chroma-location
+ * weighted average of the blended samples of its group).  Samples outside the picture are never written. */
+typedef struct hbcu_blend_config_s
+{
+    int width, height, depth;            /* frame geometry; depth 8 -> uint8 planes, 9..16 -> uint16 planes */
+    int chroma_shift_w, chroma_shift_h;  /* frame: (1,1) 4:2:0, (1,0) 4:2:2, (0,0) 4:4:4 */
+    int overlay_shift_w, overlay_shift_h;/* overlay chroma subsampling: the frame's, or (0,0) for YUVA 4:4:4 */
+    int device;
+    uint32_t chroma_coeffs[2][4];        /* hb_compute_chroma_smoothing_coefficient() of the frame's format and chroma location */
+} hbcu_blend_config_t;
+
+typedef struct hbcu_blend_overlay_s
+{
+    int x, y, width, height;             /* position in the frame (may be negative or reach past it) and size */
+    const uint8_t *planes[4];            /* HOST pointers: Y, Cb, Cr, A; only read during hbcu_blend_set_overlays() */
+    int strides[4];
+} hbcu_blend_overlay_t;
+
+typedef struct hbcu_blend_s hbcu_blend_t;
+
+int  hbcu_blend_create(hbcu_blend_t **out, const hbcu_blend_config_t *cfg);
+void hbcu_blend_destroy(hbcu_blend_t *h);
+/* the ordered overlay list of the next hbcu_blend_frames() calls.  The planes are copied into the handle's page-locked
+ * staging before this returns, then uploaded asynchronously; with changed == 0 and the same count and geometry as the
+ * previous list nothing is copied and the overlays already on the device are used again. */
+int  hbcu_blend_set_overlays(hbcu_blend_t *h, const hbcu_blend_overlay_t *list, int count, int changed);
+/* composite the current overlays, in list order, onto one frame; asynchronous.
+ *   device frames: out_frame = in_frame copied device to device, then blended; ordered behind in_frame's producer
+ *   host planes  : the rows and columns the overlays touch are copied to the device, blended and copied to out_planes
+ *                  (nothing else of out_planes is written: pass the same planes for in-place work); hbcu_blend_wait()
+ *                  returns once out_planes hold the result */
+int  hbcu_blend_frames(hbcu_blend_t *h, hbcu_frame_t *in_frame, const void *const in_planes[3], const int in_strides[3],
+                       hbcu_frame_t *out_frame, void *const out_planes[3], const int out_strides[3]);
+int  hbcu_blend_wait(hbcu_blend_t *h);
+int  hbcu_blend_sync(hbcu_blend_t *h);
+int  hbcu_blend_mark(hbcu_blend_t *h, int which);
+int  hbcu_blend_elapsed_ms(hbcu_blend_t *h, float *ms);
+/* test hook: overlay lists uploaded by all handles since load */
+uint64_t hbcu_blend_uploads(void);
+
 #ifdef __cplusplus
 }
 #endif
