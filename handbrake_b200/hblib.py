@@ -20,6 +20,9 @@ class HarnessIO(C.Structure):
         ("out_start", C.c_void_p), ("out_stop", C.c_void_p), ("out_duration", C.c_void_p),
         ("n_out", C.c_int), ("n_dropped", C.c_int), ("saw_eof", C.c_int),
         ("init_failed", C.c_int), ("vrate_num_out", C.c_int), ("vrate_den_out", C.c_int),
+        ("in_start", C.c_void_p), ("in_stop", C.c_void_p), ("in_new_chap", C.c_void_p),
+        ("vrate_num", C.c_int), ("vrate_den", C.c_int), ("cfr", C.c_int), ("collect_info", C.c_int),
+        ("out_new_chap", C.c_void_p), ("cfr_out", C.c_int), ("info_text", C.c_char * 128),
     ]
 
 
@@ -51,6 +54,9 @@ class FilterResult:
         self.init_failed = 0
         self.vrate = (0, 0)
         self.n_dropped = 0
+        self.new_chap = None
+        self.cfr = 0
+        self.info = ""
 
 
 class FilterLib:
@@ -103,9 +109,11 @@ class FilterLib:
         self.lib.hb_shim_set_cpu_count(int(n))
 
     def run(self, filters, settings, frames, pix_fmt, width, height, flags=None, combed=None,
-            max_out=None, out_scale=1):
+            max_out=None, out_scale=1, start=None, stop=None, new_chap=None, vrate=None, cfr=0, info=False):
         """filters: list of exported object names; settings: list of 'k=v:k=v' strings (or None).
-        frames: (n, frame_bytes) uint8 array.  Returns FilterResult."""
+        frames: (n, frame_bytes) uint8 array.  start / stop / new_chap: per-frame input times and chapter marks
+        (default i*3003, (i+1)*3003, i); vrate: (num, den) of the input (default 30000/1001); cfr: init->cfr;
+        info: fill FilterResult.info with the last info() text.  Returns FilterResult."""
         if isinstance(filters, str):
             filters, settings = [filters], [settings]
         frames = np.ascontiguousarray(frames, dtype=np.uint8)
@@ -129,6 +137,16 @@ class FilterLib:
         if combed is not None:
             cb = np.ascontiguousarray(combed, dtype=np.uint8); keep.append(cb)
             io.in_combed = cb.ctypes.data
+        for name, arr, dt in (("in_start", start, np.int64), ("in_stop", stop, np.int64), ("in_new_chap", new_chap, np.int32)):
+            if arr is not None:
+                a = np.ascontiguousarray(arr, dtype=dt); keep.append(a)
+                assert a.shape == (n_in,), (name, a.shape)
+                setattr(io, name, a.ctypes.data)
+        if vrate is not None:
+            io.vrate_num, io.vrate_den = int(vrate[0]), int(vrate[1])
+        io.cfr, io.collect_info = int(cfr), int(bool(info))
+        o_chap = np.zeros(cap, dtype=np.int32)
+        io.out_new_chap = o_chap.ctypes.data
         io.out, io.out_capacity = out.ctypes.data, cap
         io.out_combed, io.out_flags = o_combed.ctypes.data, o_flags.ctypes.data
         io.out_start, io.out_stop, io.out_duration = o_start.ctypes.data, o_stop.ctypes.data, o_dur.ctypes.data
@@ -144,4 +162,5 @@ class FilterLib:
         r.start, r.stop, r.duration = o_start[:k], o_stop[:k], o_dur[:k]
         r.saw_eof, r.init_failed = bool(io.saw_eof), io.init_failed
         r.vrate, r.n_dropped = (io.vrate_num_out, io.vrate_den_out), io.n_dropped
+        r.new_chap, r.cfr, r.info = o_chap[:k], io.cfr_out, io.info_text.decode()
         return r

@@ -27,6 +27,8 @@
 #include <string.h>
 #include <stdio.h>
 #include <math.h>
+#include <limits.h>
+#include <inttypes.h>
 
 #ifdef __cplusplus
 extern "C" {
@@ -497,6 +499,54 @@ extern hb_blend_object_t hb_blend;
 /* common.c:7054-7091: the per-position weights [0][x] / [1][y] of the luma samples that make up one chroma sample,
  * from the format's subsampling and the chroma location */
 void hb_compute_chroma_smoothing_coefficient(uint32_t chroma_coeffs[2][4], int pix_fmt, int chroma_location);
+
+/* ---- what the framerate shaper (vfr.c) and its motion metric (motion_metric.c) use ---- */
+#define HB_RATIONAL_REG "([0-9]+/[0-9]+)"                  /* handbrake/common.h */
+/* "num/den" (hb_dict.c: both parts digits only); 1 = key present and well-formed */
+int hb_dict_extract_rational(hb_rational_t *dst, const hb_dict_t *dict, const char *key);
+
+/* generic pointer list (common.c hb_list_*) */
+hb_list_t *hb_list_init(void);
+int        hb_list_count(const hb_list_t *l);
+void       hb_list_add(hb_list_t *l, void *p);
+void       hb_list_rem(hb_list_t *l, void *p);
+void      *hb_list_item(const hb_list_t *l, int i);
+void       hb_list_close(hb_list_t **l);
+
+/* buffer FIFO (fifo.c hb_fifo_*), single-threaded and never blocking: push appends, get returns NULL when empty,
+ * close frees what is left */
+hb_fifo_t   *hb_fifo_init(int capacity, int thresh);
+int          hb_fifo_size(hb_fifo_t *f);
+void         hb_fifo_push(hb_fifo_t *f, hb_buffer_t *b);
+hb_buffer_t *hb_fifo_get(hb_fifo_t *f);
+void         hb_fifo_close(hb_fifo_t **f);
+
+/* the job's handle and the statistics one pass leaves for the next (handbrake/handbrake.h hb_interjob_t, hb.c) */
+typedef struct hb_handle_s hb_handle_t;
+struct hb_job_s { hb_handle_t *h; };
+typedef struct hb_interjob_s
+{
+    int           sequence_id;
+    int           frame_count;
+    int           out_frame_count;
+    int64_t       total_time;
+    hb_rational_t vrate;
+} hb_interjob_t;
+hb_interjob_t *hb_interjob_get(hb_handle_t *h);
+
+/* motion metric objects (handbrake/common.h:1799-1811): the frame distance vfr.c picks frames to drop by */
+typedef struct hb_motion_metric_object_s  hb_motion_metric_object_t;
+typedef struct hb_motion_metric_private_s hb_motion_metric_private_t;   /* handbrake/hbtypes.h:44-45 */
+struct hb_motion_metric_object_s
+{
+    char                       * name;
+    int                       (* init)  (hb_motion_metric_object_t *, hb_filter_init_t *);
+    float                     (* work)  (hb_motion_metric_object_t *, hb_buffer_t *, hb_buffer_t *);
+    void                      (* close) (hb_motion_metric_object_t *);
+    hb_motion_metric_private_t * private_data;
+};
+extern hb_motion_metric_object_t hb_motion_metric;
+extern hb_filter_object_t hb_filter_vfr;
 
 extern hb_filter_object_t hb_filter_denoise;
 extern hb_filter_object_t hb_filter_detelecine;

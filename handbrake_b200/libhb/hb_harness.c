@@ -94,6 +94,7 @@ static void sink(chain_t *c, hb_buffer_t *list)
             if (io->out_start)  io->out_start[i]  = b->s.start;
             if (io->out_stop)   io->out_stop[i]   = b->s.stop;
             if (io->out_duration) io->out_duration[i] = b->s.duration;
+            if (io->out_new_chap) io->out_new_chap[i] = b->s.new_chap;
             io->n_out++;
         }
         else
@@ -156,8 +157,9 @@ int hb_harness_run_chain(int n_filters, hb_filter_object_t *const *protos,
     init.geometry.height = io->height;
     init.geometry.par.num = 1;
     init.geometry.par.den = 1;
-    init.vrate.num = 30000;
-    init.vrate.den = 1001;
+    init.vrate.num = io->vrate_num > 0 ? io->vrate_num : 30000;
+    init.vrate.den = io->vrate_den > 0 ? io->vrate_den : 1001;
+    init.cfr       = io->cfr;
     init.time_base.num = 1;
     init.time_base.den = 90000;
     init.color_prim = init.color_transfer = init.color_matrix = 1;
@@ -193,6 +195,17 @@ int hb_harness_run_chain(int n_filters, hb_filter_object_t *const *protos,
     }
     io->vrate_num_out = init.vrate.num;
     io->vrate_den_out = init.vrate.den;
+    io->cfr_out       = init.cfr;
+    io->info_text[0]  = '\0';
+    for (int k = 0; k < c.n && io->collect_info; k++)
+    {
+        hb_filter_info_t *info = c.f[k]->info ? c.f[k]->info(c.f[k]) : NULL;
+        if (info == NULL) continue;
+        if (info->human_readable_desc != NULL)
+            snprintf(io->info_text, sizeof(io->info_text), "%s", info->human_readable_desc);
+        free(info->human_readable_desc);
+        free(info);
+    }
     c.out_pix_fmt = init.pix_fmt;
     c.out_w = init.geometry.width;
     c.out_h = init.geometry.height;
@@ -203,12 +216,12 @@ int hb_harness_run_chain(int n_filters, hb_filter_object_t *const *protos,
     {
         hb_buffer_t *b = hb_harness_frame_from_packed(io->pix_fmt, io->width, io->height,
                                                       io->in + (size_t)i * frame_bytes_in);
-        b->s.start    = (int64_t)i * 3003;
-        b->s.stop     = b->s.start + 3003;
-        b->s.duration = 3003;
+        b->s.start    = io->in_start ? io->in_start[i] : (int64_t)i * 3003;
+        b->s.stop     = io->in_stop ? io->in_stop[i] : b->s.start + 3003;
+        b->s.duration = b->s.stop - b->s.start;
         b->s.flags    = io->in_flags  ? io->in_flags[i]  : PIC_FLAG_PROGRESSIVE_FRAME;
         b->s.combed   = io->in_combed ? io->in_combed[i] : HB_COMB_NONE;
-        b->s.new_chap = i;   /* lets tests check that props travel with the right frame */
+        b->s.new_chap = io->in_new_chap ? io->in_new_chap[i] : i;   /* lets tests check that props travel with the right frame */
         b->f.color_prim = init.color_prim;
         feed(&c, 0, b);
     }
@@ -234,6 +247,48 @@ int hb_harness_run(hb_filter_object_t *proto, const char *settings, hb_harness_i
     hb_filter_object_t *protos[1] = { proto };
     const char *sets[1] = { settings };
     return hb_harness_run_chain(1, protos, sets, io);
+}
+
+/* ------------------------------------------------------------------ */
+/* motion metric objects                                                */
+/* ------------------------------------------------------------------ */
+static hb_buffer_t *luma_frame(int pix_fmt, int w, int h, int pad, const uint8_t *src)
+{
+    const int line = av_image_get_linesize(pix_fmt, w, 0), stride = line + pad;
+    hb_buffer_t *b = hb_buffer_init(stride * h);
+    if (b == NULL) return NULL;
+    b->s.type = FRAME_BUF;
+    b->f.fmt = pix_fmt;
+    b->f.width = w;
+    b->f.height = h;
+    b->plane[0].data = b->data;
+    b->plane[0].stride = stride;
+    b->plane[0].width = w;
+    b->plane[0].height = h;
+    b->plane[0].size = stride * h;
+    for (int y = 0; y < h; y++)
+        memcpy(b->data + (size_t)y * stride, src + (size_t)y * line, line);
+    return b;
+}
+
+float hb_harness_motion_metric(hb_motion_metric_object_t *proto, int pix_fmt, int w, int h, int pad,
+                               const uint8_t *a, const uint8_t *b)
+{
+    hb_motion_metric_object_t m = *proto;
+    m.private_data = NULL;
+    hb_filter_init_t init;
+    memset(&init, 0, sizeof(init));
+    init.pix_fmt = pix_fmt;
+    init.geometry.width = w;
+    init.geometry.height = h;
+    if (m.init(&m, &init) != 0)
+        return NAN;
+    hb_buffer_t *fa = luma_frame(pix_fmt, w, h, pad, a), *fb = luma_frame(pix_fmt, w, h, pad, b);
+    const float v = (fa && fb) ? m.work(&m, fa, fb) : NAN;
+    hb_buffer_close(&fa);
+    hb_buffer_close(&fb);
+    m.close(&m);
+    return v;
 }
 
 /* ------------------------------------------------------------------ */

@@ -27,6 +27,17 @@ typedef struct hb_harness_io_s
     int             saw_eof;
     int             init_failed; /* bit k set: filter k's init() returned non-zero */
     int             vrate_num_out, vrate_den_out;
+    /* input, optional (NULL / 0: frame i runs from i*3003 to (i+1)*3003 with new_chap = i, at 30000/1001, cfr 0) */
+    const int64_t  *in_start;    /* per-frame s.start */
+    const int64_t  *in_stop;     /* per-frame s.stop */
+    const int      *in_new_chap; /* per-frame s.new_chap */
+    int             vrate_num, vrate_den;   /* init->vrate */
+    int             cfr;         /* init->cfr */
+    int             collect_info;   /* fill info_text */
+    /* output */
+    int            *out_new_chap;
+    int             cfr_out;     /* init->cfr after every filter's init() */
+    char            info_text[128];   /* human_readable_desc of the last filter whose info() gives one */
 } hb_harness_io_t;
 
 size_t       hb_harness_frame_bytes(int pix_fmt, int w, int h);
@@ -35,6 +46,12 @@ void         hb_harness_frame_to_packed(const hb_buffer_t *b, uint8_t *dst);
 int hb_harness_run(hb_filter_object_t *proto, const char *settings, hb_harness_io_t *io);
 int hb_harness_run_chain(int n_filters, hb_filter_object_t *const *protos,
                          const char *const *settings, hb_harness_io_t *io);
+
+/* one motion metric object (hb_motion_metric ...) on one pair of frames: init() with the format and geometry, work() on
+ * frames a and b (packed planar, see above) whose luma rows are `pad` bytes longer than the picture, close().  Returns
+ * work()'s value; NaN when init() fails. */
+float hb_harness_motion_metric(hb_motion_metric_object_t *proto, int pix_fmt, int w, int h, int pad,
+                               const uint8_t *a, const uint8_t *b);
 
 /* ---- a stand-in for libhb's render_sub filter (rendersub.c): burns a per-frame schedule of overlays into the frames
  * through a blend object (hb_blend, hb_blend_cuda ...), calling its init / work / close the way rendersub does ---- */

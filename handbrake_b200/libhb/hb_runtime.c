@@ -14,6 +14,7 @@
 #define _GNU_SOURCE
 #include "handbrake/handbrake.h"
 
+#include <ctype.h>
 #include <pthread.h>
 #include <sched.h>
 #include <stdarg.h>
@@ -705,6 +706,92 @@ int hb_dict_extract_string(char **dst, const hb_dict_t *dict, const char *key)
     *dst = strdup(e->val);
     return 1;
 }
+
+int hb_dict_extract_rational(hb_rational_t *dst, const hb_dict_t *dict, const char *key)
+{
+    const dict_entry_t *e = dict_find(dict, key);
+    if (e == NULL || dst == NULL) return 0;
+    const char *slash = strchr(e->val, '/');
+    if (slash == NULL || !isdigit((unsigned char)e->val[0]) || !isdigit((unsigned char)slash[1]))
+        return 0;
+    /* the parts between the first two slashes must be whole numbers */
+    const char *end2 = strchr(slash + 1, '/');
+    char *num_end, *den_end;
+    const int num = (int)strtol(e->val, &num_end, 0);
+    const int den = (int)strtol(slash + 1, &den_end, 0);
+    if (num_end != slash || (end2 ? den_end != end2 : *den_end != '\0')) return 0;
+    dst->num = num;
+    dst->den = den;
+    return 1;
+}
+
+/* ------------------------------------------------------------------ */
+/* lists, FIFOs, interjob                                               */
+/* ------------------------------------------------------------------ */
+struct hb_list_s { void **items; int count, cap; };
+
+hb_list_t *hb_list_init(void) { return calloc(1, sizeof(hb_list_t)); }
+int hb_list_count(const hb_list_t *l) { return l ? l->count : 0; }
+
+void hb_list_add(hb_list_t *l, void *p)
+{
+    if (l == NULL || p == NULL) return;
+    if (l->count == l->cap)
+    {
+        const int cap = l->cap ? 2 * l->cap : 16;
+        void **items = realloc(l->items, sizeof(void *) * cap);
+        if (items == NULL) return;
+        l->items = items;
+        l->cap = cap;
+    }
+    l->items[l->count++] = p;
+}
+
+void hb_list_rem(hb_list_t *l, void *p)
+{
+    if (l == NULL) return;
+    for (int i = 0; i < l->count; i++)
+        if (l->items[i] == p)
+        {
+            memmove(&l->items[i], &l->items[i + 1], sizeof(void *) * (l->count - i - 1));
+            l->count--;
+            return;
+        }
+}
+
+void *hb_list_item(const hb_list_t *l, int i)
+{
+    return (l == NULL || i < 0 || i >= l->count) ? NULL : l->items[i];
+}
+
+void hb_list_close(hb_list_t **l)
+{
+    if (l == NULL || *l == NULL) return;
+    free((*l)->items);
+    free(*l);
+    *l = NULL;
+}
+
+struct hb_fifo_s { hb_buffer_list_t list; };
+
+hb_fifo_t *hb_fifo_init(int capacity, int thresh)
+{
+    (void)capacity; (void)thresh;
+    return calloc(1, sizeof(hb_fifo_t));
+}
+int hb_fifo_size(hb_fifo_t *f) { return f ? hb_buffer_list_count(&f->list) : 0; }
+void hb_fifo_push(hb_fifo_t *f, hb_buffer_t *b) { if (f && b) hb_buffer_list_append(&f->list, b); }
+hb_buffer_t *hb_fifo_get(hb_fifo_t *f) { return f ? hb_buffer_list_rem_head(&f->list) : NULL; }
+void hb_fifo_close(hb_fifo_t **f)
+{
+    if (f == NULL || *f == NULL) return;
+    hb_buffer_list_close(&(*f)->list);
+    free(*f);
+    *f = NULL;
+}
+
+struct hb_handle_s { hb_interjob_t interjob; };
+hb_interjob_t *hb_interjob_get(hb_handle_t *h) { return h ? &h->interjob : NULL; }
 
 hb_dict_t *hb_parse_filter_settings(const char *settings)
 {

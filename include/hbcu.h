@@ -501,6 +501,47 @@ int  hbcu_blend_elapsed_ms(hbcu_blend_t *h, float *ms);
 /* test hook: overlay lists uploaded by all handles since load */
 uint64_t hbcu_blend_uploads(void);
 
+/* ------------------------------------------------------------------------- */
+/* motion metric  replaces the x86 metric of libhb/motion_metric.c              */
+/*              (approximate_frame_data, sse_block16, motion_metric{,_fast}):   */
+/*              the frame-to-frame distance vfr.c drops CFR / PFR frames by     */
+/* ------------------------------------------------------------------------- */
+/* Gamma-weighted SSE over whole 16x16 blocks of luma; each block's sum wraps in uint32 and the block sums add into a
+ * uint64, exactly as the reference's x86 code.  On the fast path (the reference takes it when the job's geometry is
+ * at least 1920 wide or 1080 high) both images are first reduced to width/4 x height/4 by nested rounding averages of
+ * 4x4 cells.  The handle returns that uint64 sum; the caller divides, (float)sum / (w * h), with w x h the (reduced)
+ * geometry.  Every frame is read once: a new frame B becomes a "slot" (on the fast path its reduced image, otherwise
+ * B's luma itself: a reference on a device frame or a device copy of host luma) that later frames compare against. */
+typedef struct hbcu_motion_metric_config_s
+{
+    int width, height;                   /* luma geometry of every frame */
+    int depth;                           /* 8 -> uint8 luma, 9..16 -> uint16 */
+    int fast;                            /* compare the 4x4-reduced images */
+    int device;
+    int slots;                           /* frames kept to be compared against */
+    int results;                         /* result slots */
+    const unsigned *gamma_lut;           /* (1 << depth) entries, built by the host as motion_metric.c's build_gamma_lut */
+} hbcu_motion_metric_config_t;
+
+typedef struct hbcu_motion_metric_s hbcu_motion_metric_t;
+
+int  hbcu_motion_metric_create(hbcu_motion_metric_t **out, const hbcu_motion_metric_config_t *cfg);
+void hbcu_motion_metric_destroy(hbcu_motion_metric_t *h);
+/* frame B becomes slot `slot`; when a_slot >= 0, the sum of B against the frame in slot `a_slot` (filled by an earlier
+ * call) is queued into result slot `result`.  B is a device frame (luma plane read in place; queued behind the frame's
+ * producer, recorded as one of its readers, no host wait) or, with frame == NULL, host luma with its stride (copied to
+ * the device before this returns: the caller may free it right after). */
+int  hbcu_motion_metric_enqueue(hbcu_motion_metric_t *h, int slot, int a_slot, int result,
+                                hbcu_frame_t *frame, const void *luma, int stride);
+/* waits for result slot `result` only and returns its sum */
+int  hbcu_motion_metric_result(hbcu_motion_metric_t *h, int result, uint64_t *sum);
+int  hbcu_motion_metric_sync(hbcu_motion_metric_t *h);
+int  hbcu_motion_metric_mark(hbcu_motion_metric_t *h, int which);
+int  hbcu_motion_metric_elapsed_ms(hbcu_motion_metric_t *h, float *ms);
+/* test hooks, all handles since load: result reads that had to block, and metric kernel launches */
+uint64_t hbcu_motion_metric_waits(void);
+uint64_t hbcu_motion_metric_launches(void);
+
 #ifdef __cplusplus
 }
 #endif
