@@ -13,6 +13,14 @@
 // crossing the right or bottom edge in the subsample path, an odd negative position or an overlay wider than the frame
 // in the plain path); here nothing outside the picture is ever written.
 //
+// Semi-planar 4:2:0 frames (NV12, P010, P016: plane 1 holds Cb/Cr pairs) follow blend.c's own *bi* functions
+// (blend8onbi8 / blend8onbi1x, blend.c:606-786; blend_subsample_8onbi8 / blend_subsample_8onbi1x, blend.c:142-234,
+// 330-422), which are not the planar ones with another address:
+//   - above 8 bits an overlay sample v enters as av_bswap16(v) = v << 8, whatever the depth; alpha is still
+//     << (depth - 8) and max still (256 << (depth - 8)) - 1 (blend.c:193, 214-217, 747, 778-783);
+//   - blend_subsample_8onbi8's group loops do not stop at the overlay's right / bottom edge (blend.c:388-390): every
+//     sample of the group is weighted into accu_c, the ones outside the overlay with the frame's unblended chroma.
+//
 // Thread mapping: one thread per chroma group (2x2, 2x1 or 1x1 luma samples and the chroma sample they share) of the
 // union of the rectangles the overlays can touch; each thread loads its samples once, runs through all overlay
 // descriptors in order and stores once.  A frame is one launch whatever the number of overlays.  No two groups share a
@@ -54,6 +62,8 @@ struct BlendArgs
     int W, H, CW, CH;
     int ws, hs;
     int shift;
+    int oshift;               // overlay samples enter as v << oshift: shift, or 8 on a semi-planar frame above 8 bits
+    int full_groups;          // blend_subsample_8onbi8: weigh every sample of a group (blend.c:388-390)
     unsigned maxv;
     unsigned c0[4], c1[4];
     int gx0, gy0, gw;
@@ -74,8 +84,9 @@ __device__ __forceinline__ void st(uint8_t *plane, int pitch, int x, int y, unsi
     reinterpret_cast<T *>(plane + (size_t)y * pitch)[x] = (T)v;
 }
 
-// SUB: blend_subsample_8on{8,1x}; else blend8on{8,1x}.  T: the frame's sample type.
-template <typename T, bool SUB>
+// SUB: blend_subsample_8on{8,1x}; else blend8on{8,1x}.  NV: the *bi* variants, Cb/Cr interleaved in plane 1.
+// T: the frame's sample type.
+template <typename T, bool SUB, bool NV>
 __global__ void __launch_bounds__(kThreads) blend_kernel(const BlendArgs a)
 {
     const int gx = a.gx0 + blockIdx.x * kThreads + threadIdx.x;
@@ -84,14 +95,14 @@ __global__ void __launch_bounds__(kThreads) blend_kernel(const BlendArgs a)
     const int sw = 1 << a.ws, sh = 1 << a.hs;
     const int X = gx << a.ws, Y = gy << a.hs;
     const unsigned maxv = a.maxv, half = maxv >> 1;
-    const int shift = a.shift;
+    const int shift = a.shift, oshift = a.oshift;
 
     unsigned yv[2][2] = {{0, 0}, {0, 0}};
     for (int j = 0; j < sh; j++)
         for (int i = 0; i < sw; i++)
             if (X + i < a.W && Y + j < a.H) yv[j][i] = ld<T>(a.plane[0], a.pitch[0], X + i, Y + j);
-    unsigned u = ld<T>(a.plane[1], a.pitch[1], gx, gy);
-    unsigned v = ld<T>(a.plane[2], a.pitch[2], gx, gy);
+    unsigned u = NV ? ld<T>(a.plane[1], a.pitch[1], 2 * gx, gy) : ld<T>(a.plane[1], a.pitch[1], gx, gy);
+    unsigned v = NV ? ld<T>(a.plane[1], a.pitch[1], 2 * gx + 1, gy) : ld<T>(a.plane[2], a.pitch[2], gx, gy);
 
     for (int k = 0; k < a.n; k++)
     {
@@ -108,7 +119,7 @@ __global__ void __launch_bounds__(kThreads) blend_kernel(const BlendArgs a)
                     if (X + i < a.W && Y + j < a.H && ox >= 0 && ox < width && oy >= 0 && oy < height)
                     {
                         const unsigned alpha = (unsigned)oA[oy * o.stride[3] + ox] << shift;
-                        yv[j][i] = (yv[j][i] * (maxv - alpha) + ((unsigned)oY[oy * o.stride[0] + ox] << shift) * alpha + half) / maxv;
+                        yv[j][i] = (yv[j][i] * (maxv - alpha) + ((unsigned)oY[oy * o.stride[0] + ox] << oshift) * alpha + half) / maxv;
                     }
                 }
             // the chroma of a group is visited when its top-left luma sample is inside the loop (blend.c:81-102)
@@ -117,17 +128,17 @@ __global__ void __launch_bounds__(kThreads) blend_kernel(const BlendArgs a)
             if (X >= x0c && ox < width && Y >= y0c && oy < height)
             {
                 unsigned accu_a = 0, accu_b = 0, accu_c = 0;
-                for (int yz = 0; yz < sh && oy + yz < height; yz++)
-                    for (int xz = 0; xz < sw && ox + xz < width; xz++)
+                for (int yz = 0; yz < sh && (a.full_groups || oy + yz < height); yz++)
+                    for (int xz = 0; xz < sw && (a.full_groups || ox + xz < width); xz++)
                     {
                         const unsigned coeff = a.c0[xz] * a.c1[yz];
                         unsigned ru = u, rv = v;
-                        if (ox + xz >= 0 && oy + yz >= 0)
+                        if (ox + xz >= 0 && oy + yz >= 0 && ox + xz < width && oy + yz < height)
                         {
                             const int oxz = ox + xz, oyz = oy + yz;
                             const unsigned alpha = (unsigned)oA[oyz * o.stride[3] + oxz] << shift;
-                            ru = (ru * (maxv - alpha) + ((unsigned)oU[oyz * o.stride[1] + oxz] << shift) * alpha + half) / maxv;
-                            rv = (rv * (maxv - alpha) + ((unsigned)oV[oyz * o.stride[2] + oxz] << shift) * alpha + half) / maxv;
+                            ru = (ru * (maxv - alpha) + ((unsigned)oU[oyz * o.stride[1] + oxz] << oshift) * alpha + half) / maxv;
+                            rv = (rv * (maxv - alpha) + ((unsigned)oV[oyz * o.stride[2] + oxz] << oshift) * alpha + half) / maxv;
                         }
                         accu_a += coeff * ru;
                         accu_b += coeff * rv;
@@ -150,7 +161,7 @@ __global__ void __launch_bounds__(kThreads) blend_kernel(const BlendArgs a)
                     if (X + i < a.W && Y + j < a.H && xx >= x0 && xx < ww && yy >= y0 && yy < hh)
                     {
                         const unsigned alpha = (unsigned)oA[yy * o.stride[3] + xx] << shift;
-                        yv[j][i] = (yv[j][i] * (maxv - alpha) + ((unsigned)oY[yy * o.stride[0] + xx] << shift) * alpha) / maxv;
+                        yv[j][i] = (yv[j][i] * (maxv - alpha) + ((unsigned)oY[yy * o.stride[0] + xx] << oshift) * alpha) / maxv;
                     }
                 }
             // blend.c:486-508: chroma row yy lands at yy + (top >> hshift) (arithmetic shift), alpha from the top-left
@@ -159,8 +170,8 @@ __global__ void __launch_bounds__(kThreads) blend_kernel(const BlendArgs a)
             if (xx >= (x0 >> a.ws) && xx < (ww >> a.ws) && yy >= (y0 >> a.hs) && yy < (hh >> a.hs))
             {
                 const unsigned alpha = (unsigned)oA[(yy << a.hs) * o.stride[3] + (xx << a.ws)] << shift;
-                u = (u * (maxv - alpha) + ((unsigned)oU[yy * o.stride[1] + xx] << shift) * alpha) / maxv;
-                v = (v * (maxv - alpha) + ((unsigned)oV[yy * o.stride[2] + xx] << shift) * alpha) / maxv;
+                u = (u * (maxv - alpha) + ((unsigned)oU[yy * o.stride[1] + xx] << oshift) * alpha) / maxv;
+                v = (v * (maxv - alpha) + ((unsigned)oV[yy * o.stride[2] + xx] << oshift) * alpha) / maxv;
             }
         }
     }
@@ -168,8 +179,16 @@ __global__ void __launch_bounds__(kThreads) blend_kernel(const BlendArgs a)
     for (int j = 0; j < sh; j++)
         for (int i = 0; i < sw; i++)
             if (X + i < a.W && Y + j < a.H) st<T>(a.plane[0], a.pitch[0], X + i, Y + j, yv[j][i]);
-    st<T>(a.plane[1], a.pitch[1], gx, gy, u);
-    st<T>(a.plane[2], a.pitch[2], gx, gy, v);
+    if (NV)
+    {
+        st<T>(a.plane[1], a.pitch[1], 2 * gx, gy, u);
+        st<T>(a.plane[1], a.pitch[1], 2 * gx + 1, gy, v);
+    }
+    else
+    {
+        st<T>(a.plane[1], a.pitch[1], gx, gy, u);
+        st<T>(a.plane[2], a.pitch[2], gx, gy, v);
+    }
 }
 
 struct Slot
@@ -186,6 +205,8 @@ struct hbcu_blend_s
 {
     hbcu_blend_config_t cfg;
     int bps, cw, ch, subsample;
+    int nplanes;                               // 3, or 2 for a semi-planar frame (plane 2 absent: 0 rows of 0 bytes)
+    int sample_bytes[3];                       // bytes per sample position of each plane (a Cb/Cr pair counts once)
     int row_bytes[3], pitch[3];
     size_t plane_off[3], frame_bytes;
     uint8_t *staging = nullptr;                // host frames: the band the overlays touch is blended here
@@ -200,7 +221,7 @@ namespace {
 bool frame_fits(const hbcu_blend_s *h, const hbcu_frame_t *f)
 {
     if (f->device != h->cfg.device) return false;
-    const int rows[3] = {h->cfg.height, h->ch, h->ch};
+    const int rows[3] = {h->cfg.height, h->ch, h->nplanes == 3 ? h->ch : 0};
     for (int p = 0; p < 3; p++)
         if (f->row_bytes[p] != h->row_bytes[p] || f->rows[p] != rows[p]) return false;
     return true;
@@ -234,6 +255,8 @@ int launch(hbcu_blend_s *h, uint8_t *const planes[3], const int pitches[3], int 
     a.W = h->cfg.width; a.H = h->cfg.height; a.CW = h->cw; a.CH = h->ch;
     a.ws = h->cfg.chroma_shift_w; a.hs = h->cfg.chroma_shift_h;
     a.shift = h->cfg.depth - 8;
+    a.oshift = (h->cfg.interleaved_chroma && h->bps == 2) ? 8 : a.shift;
+    a.full_groups = h->cfg.interleaved_chroma && h->bps == 1 && h->subsample;
     a.maxv = (256u << a.shift) - 1;
     for (int i = 0; i < 4; i++) { a.c0[i] = h->cfg.chroma_coeffs[0][i]; a.c1[i] = h->cfg.chroma_coeffs[1][i]; }
     a.gx0 = gx0; a.gy0 = gy0; a.gw = gx1 - gx0;
@@ -241,8 +264,16 @@ int launch(hbcu_blend_s *h, uint8_t *const planes[3], const int pitches[3], int 
     a.blob = s.dev;
     a.n = (int)s.desc.size();
     const dim3 grid((a.gw + kThreads - 1) / kThreads, gy1 - gy0);
-    if (h->bps == 1) { if (h->subsample) blend_kernel<uint8_t, true><<<grid, kThreads, 0, h->st>>>(a); else blend_kernel<uint8_t, false><<<grid, kThreads, 0, h->st>>>(a); }
-    else             { if (h->subsample) blend_kernel<uint16_t, true><<<grid, kThreads, 0, h->st>>>(a); else blend_kernel<uint16_t, false><<<grid, kThreads, 0, h->st>>>(a); }
+    if (h->cfg.interleaved_chroma)
+    {
+        if (h->bps == 1) { if (h->subsample) blend_kernel<uint8_t, true, true><<<grid, kThreads, 0, h->st>>>(a); else blend_kernel<uint8_t, false, true><<<grid, kThreads, 0, h->st>>>(a); }
+        else             { if (h->subsample) blend_kernel<uint16_t, true, true><<<grid, kThreads, 0, h->st>>>(a); else blend_kernel<uint16_t, false, true><<<grid, kThreads, 0, h->st>>>(a); }
+    }
+    else
+    {
+        if (h->bps == 1) { if (h->subsample) blend_kernel<uint8_t, true, false><<<grid, kThreads, 0, h->st>>>(a); else blend_kernel<uint8_t, false, false><<<grid, kThreads, 0, h->st>>>(a); }
+        else             { if (h->subsample) blend_kernel<uint16_t, true, false><<<grid, kThreads, 0, h->st>>>(a); else blend_kernel<uint16_t, false, false><<<grid, kThreads, 0, h->st>>>(a); }
+    }
     HBCU_CHECK(cudaGetLastError());
     hbcu::count_launch();
     return 0;
@@ -263,10 +294,12 @@ int hbcu_blend_create(hbcu_blend_t **out, const hbcu_blend_config_t *cfg)
     const int ws = cfg->chroma_shift_w, hs = cfg->chroma_shift_h, ows = cfg->overlay_shift_w, ohs = cfg->overlay_shift_h;
     const bool frame_ok = (ws == 1 && hs == 1) || (ws == 1 && hs == 0) || (ws == 0 && hs == 0);
     const bool overlay_ok = (ows == ws && ohs == hs) || (ows == 0 && ohs == 0);
-    if (cfg->width < 1 || cfg->height < 1 || cfg->depth < 8 || cfg->depth > 16 || !frame_ok || !overlay_ok)
+    // the semi-planar formats of NVDEC are 4:2:0 only
+    const bool interleave_ok = cfg->interleaved_chroma == 0 || (cfg->interleaved_chroma == 1 && ws == 1 && hs == 1);
+    if (cfg->width < 1 || cfg->height < 1 || cfg->depth < 8 || cfg->depth > 16 || !frame_ok || !overlay_ok || !interleave_ok)
     {
-        set_error("blend_create: unsupported geometry %dx%d depth %d, frame chroma shifts %d,%d, overlay %d,%d",
-                  cfg->width, cfg->height, cfg->depth, ws, hs, ows, ohs);
+        set_error("blend_create: unsupported geometry %dx%d depth %d, frame chroma shifts %d,%d, overlay %d,%d, interleaved chroma %d",
+                  cfg->width, cfg->height, cfg->depth, ws, hs, ows, ohs, cfg->interleaved_chroma);
         return -1;
     }
     const int cw = -((-cfg->width) >> ws), ch = -((-cfg->height) >> hs);
@@ -300,10 +333,12 @@ int hbcu_blend_create(hbcu_blend_t **out, const hbcu_blend_config_t *cfg)
     h->cw = cw;
     h->ch = ch;
     h->subsample = subsample;
+    h->nplanes = cfg->interleaved_chroma ? 2 : 3;
     size_t off = 0;
     for (int p = 0; p < 3; p++)
     {
-        h->row_bytes[p] = (p ? cw : cfg->width) * h->bps;
+        h->sample_bytes[p] = p >= h->nplanes ? 0 : (p == 1 && cfg->interleaved_chroma ? 2 : 1) * h->bps;
+        h->row_bytes[p] = (p ? cw : cfg->width) * h->sample_bytes[p];
         h->pitch[p] = (h->row_bytes[p] + 63) / 64 * 64;
         h->plane_off[p] = off;
         off += (size_t)h->pitch[p] * (p ? ch : cfg->height);
@@ -434,7 +469,7 @@ int hbcu_blend_frames(hbcu_blend_t *h, hbcu_frame_t *in_frame, const void *const
     {
         if (hbcu::frame_begin_read(in_frame, h->st) != 0) return -1;
         if (hbcu::frame_begin_write(out_frame, h->st) != 0) return -1;
-        for (int p = 0; p < 3; p++)
+        for (int p = 0; p < h->nplanes; p++)
             HBCU_CHECK(cudaMemcpy2DAsync(out_frame->plane[p], out_frame->stride[p], in_frame->plane[p], in_frame->stride[p],
                                          h->row_bytes[p], in_frame->rows[p], cudaMemcpyDeviceToDevice, h->st));
         if (hbcu::frame_end_read(in_frame, h->st) != 0) return -1;
@@ -446,22 +481,24 @@ int hbcu_blend_frames(hbcu_blend_t *h, hbcu_frame_t *in_frame, const void *const
         // the band of rows and columns the overlays touch, per plane: luma in samples, chroma in groups
         const int x0[3] = {gx0 << ws, gx0, gx0}, x1[3] = {std::min(h->cfg.width, gx1 << ws), gx1, gx1};
         const int y0[3] = {gy0 << hs, gy0, gy0}, y1[3] = {std::min(h->cfg.height, gy1 << hs), gy1, gy1};
-        uint8_t *dplanes[3];
-        for (int p = 0; p < 3; p++)
+        uint8_t *dplanes[3] = {nullptr, nullptr, nullptr};
+        for (int p = 0; p < h->nplanes; p++)
         {
+            const int sb = h->sample_bytes[p];
             dplanes[p] = h->staging + h->plane_off[p];
-            const size_t dst_off = (size_t)y0[p] * h->pitch[p] + (size_t)x0[p] * h->bps;
-            const size_t src_off = (size_t)y0[p] * in_strides[p] + (size_t)x0[p] * h->bps;
+            const size_t dst_off = (size_t)y0[p] * h->pitch[p] + (size_t)x0[p] * sb;
+            const size_t src_off = (size_t)y0[p] * in_strides[p] + (size_t)x0[p] * sb;
             HBCU_CHECK(cudaMemcpy2DAsync(dplanes[p] + dst_off, h->pitch[p], (const uint8_t *)in_planes[p] + src_off, in_strides[p],
-                                         (size_t)(x1[p] - x0[p]) * h->bps, y1[p] - y0[p], cudaMemcpyHostToDevice, h->st));
+                                         (size_t)(x1[p] - x0[p]) * sb, y1[p] - y0[p], cudaMemcpyHostToDevice, h->st));
         }
         if (launch(h, dplanes, h->pitch, gx0, gx1, gy0, gy1) != 0) return -1;
-        for (int p = 0; p < 3; p++)
+        for (int p = 0; p < h->nplanes; p++)
         {
-            const size_t dev_off = (size_t)y0[p] * h->pitch[p] + (size_t)x0[p] * h->bps;
-            const size_t host_off = (size_t)y0[p] * out_strides[p] + (size_t)x0[p] * h->bps;
+            const int sb = h->sample_bytes[p];
+            const size_t dev_off = (size_t)y0[p] * h->pitch[p] + (size_t)x0[p] * sb;
+            const size_t host_off = (size_t)y0[p] * out_strides[p] + (size_t)x0[p] * sb;
             HBCU_CHECK(cudaMemcpy2DAsync((uint8_t *)out_planes[p] + host_off, out_strides[p], dplanes[p] + dev_off, h->pitch[p],
-                                         (size_t)(x1[p] - x0[p]) * h->bps, y1[p] - y0[p], cudaMemcpyDeviceToHost, h->st));
+                                         (size_t)(x1[p] - x0[p]) * sb, y1[p] - y0[p], cudaMemcpyDeviceToHost, h->st));
         }
     }
     HBCU_CHECK(cudaEventRecord(h->slot[h->cur].done, h->st));

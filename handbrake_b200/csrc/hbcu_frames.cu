@@ -26,6 +26,9 @@ std::mutex g_reader_lock;       // makes a reader's wait-then-record on `consume
 hbcu_frame_s *g_frame_free = nullptr;
 long g_frames_alive = 0;          // frames handed out and not yet released (leak check for the tests)
 
+// a semi-planar frame (NV12, P010, P016) has no third plane: it is given as 0 rows of 0 bytes
+bool absent_plane(int p, const int row_bytes[3], const int rows[3]) { return p == 2 && rows[2] == 0 && row_bytes[2] == 0; }
+
 bool same_geometry(const hbcu_frame_s *f, int device, const int row_bytes[3], const int rows[3], const int strides[3])
 {
     if (f->device != device) return false;
@@ -90,8 +93,11 @@ int hbcu_frame_alloc(hbcu_frame_t **out, int device, const int row_bytes[3], con
         return -1;
     }
     *out = nullptr;
+    int stride_of[3];                                   // an absent plane's stride is 0 whatever was passed (pool key)
     for (int p = 0; p < 3; p++)
     {
+        stride_of[p] = absent_plane(p, row_bytes, rows) ? 0 : strides[p];
+        if (absent_plane(p, row_bytes, rows)) continue;
         if (row_bytes[p] <= 0 || rows[p] <= 0 || strides[p] < row_bytes[p] || (strides[p] % 16) != 0)
         {
             hbcu::set_error("hbcu_frame_alloc: plane %d: %d bytes x %d rows, stride %d (strides must be multiples of 16)", p,
@@ -99,6 +105,7 @@ int hbcu_frame_alloc(hbcu_frame_t **out, int device, const int row_bytes[3], con
             return -1;
         }
     }
+    strides = stride_of;
     {
         std::lock_guard<std::mutex> g(g_frame_lock);
         hbcu_frame_s **link = &g_frame_free;
@@ -170,7 +177,7 @@ int hbcu_frame_alloc(hbcu_frame_t **out, int device, const int row_bytes[3], con
     off = 0;
     for (int p = 0; p < 3; p++)
     {
-        f->plane[p] = f->base + off;
+        f->plane[p] = absent_plane(p, row_bytes, rows) ? nullptr : f->base + off;
         off += (size_t)strides[p] * rows[p];
     }
     {
@@ -226,7 +233,8 @@ int hbcu_frame_wrap(hbcu_frame_t **out, int device, void *const dplanes[3], cons
         return -1;
     }
     *out = nullptr;
-    for (int p = 0; p < 3; p++)
+    const bool two_planes = absent_plane(2, row_bytes, rows) && dplanes[2] == nullptr;
+    for (int p = 0; p < (two_planes ? 2 : 3); p++)
     {
         if (dplanes[p] == nullptr || ((uintptr_t)dplanes[p] % 16) != 0 || row_bytes[p] <= 0 || rows[p] <= 0 ||
             strides[p] < row_bytes[p] || (strides[p] % 16) != 0)
@@ -262,7 +270,7 @@ int hbcu_frame_wrap(hbcu_frame_t **out, int device, void *const dplanes[3], cons
         f->plane[p] = (uint8_t *)dplanes[p];
         f->row_bytes[p] = row_bytes[p];
         f->rows[p] = rows[p];
-        f->stride[p] = strides[p];
+        f->stride[p] = (two_planes && p == 2) ? 0 : strides[p];
     }
     f->ready = f->consumed = nullptr;
     f->next = nullptr;
@@ -382,6 +390,7 @@ static bool host_matches_frame(const hbcu_frame_t *f, const void *const planes[3
     size_t off = 0;
     for (int p = 0; p < 3; p++)
     {
+        if (f->plane[p] == nullptr) continue;                // the absent third plane of a semi-planar frame
         if (strides[p] != f->stride[p] || (const uint8_t *)planes[p] != (const uint8_t *)planes[0] + off) return false;
         off += (size_t)f->stride[p] * f->rows[p];
     }
@@ -410,6 +419,7 @@ static int xfer_copy(hbcu_xfer_t *x, int64_t ticket, hbcu_frame_t *f, void *cons
     {
         for (int p = 0; p < 3; p++)
         {
+            if (f->plane[p] == nullptr) continue;
             if (download)
                 HBCU_CHECK(cudaMemcpy2DAsync(planes[p], (size_t)strides[p], f->plane[p], (size_t)f->stride[p], (size_t)f->row_bytes[p],
                                              (size_t)f->rows[p], kind, x->st));

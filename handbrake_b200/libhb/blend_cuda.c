@@ -3,8 +3,9 @@
  *
  * Same init / work / close contract:
  *   - init takes the frame's geometry, format, chroma location and the overlay format; it fails (non-zero) for a
- *     combination blend.c's CUDA twin does not support (semi-planar frames, a subsampled overlay on a frame with other
- *     subsampling) and when there is no usable device, so that the caller can take hb_blend instead;
+ *     combination blend.c's CUDA twin does not support (a semi-planar frame other than 4:2:0, a subsampled overlay on
+ *     a frame with other subsampling) and when there is no usable device, so that the caller can take hb_blend
+ *     instead.  Semi-planar 4:2:0 frames (NV12, P010, P016, what NVDEC decodes into) take blend.c's *bi* paths;
  *   - work composites the overlays in list order.  No overlays: the input buffer comes back as it is, nothing runs on
  *     the GPU (blend.c:856-859).  A host frame is blended in place (duplicated first if it is not writable,
  *     blend.c:861-865) and is finished when work returns.  A device frame is never written (frames are written once):
@@ -45,7 +46,10 @@ static int blend_cuda_init(hb_blend_object_t *object, int in_width, int in_heigh
     object->private_data = NULL;
     const AVPixFmtDescriptor *in_desc = av_pix_fmt_desc_get(in_pix_fmt);
     const AVPixFmtDescriptor *ov_desc = av_pix_fmt_desc_get(overlay_pix_fmt);
-    if (in_desc == NULL || ov_desc == NULL || av_pix_fmt_count_planes(in_pix_fmt) != 3 || in_desc->nb_components != 3 ||
+    const int in_planes = av_pix_fmt_count_planes(in_pix_fmt);
+    /* blend.c:817-842 picks the *bi* functions by plane count; the semi-planar formats in use for them are 4:2:0 */
+    const int semi_planar = in_desc != NULL && in_planes == 2 && in_desc->log2_chroma_w == 1 && in_desc->log2_chroma_h == 1;
+    if (in_desc == NULL || ov_desc == NULL || (in_planes != 3 && !semi_planar) || in_desc->nb_components != 3 ||
         av_pix_fmt_count_planes(overlay_pix_fmt) != 4 || ov_desc->comp[0].depth != 8 ||
         in_desc->comp[0].depth < 8 || in_desc->comp[0].depth > 16)
     {
@@ -74,6 +78,7 @@ static int blend_cuda_init(hb_blend_object_t *object, int in_width, int in_heigh
     cfg.overlay_shift_w = ov_desc->log2_chroma_w;
     cfg.overlay_shift_h = ov_desc->log2_chroma_h;
     cfg.device          = pv->device = hbcu_env_device();
+    cfg.interleaved_chroma = semi_planar;
     hb_compute_chroma_smoothing_coefficient(cfg.chroma_coeffs, in_pix_fmt, in_chroma_location);
     if (hbcu_blend_create(&pv->gpu, &cfg) != 0)
     {
@@ -164,9 +169,9 @@ static hb_buffer_t *blend_cuda_work(hb_blend_object_t *object, hb_buffer_t *in, 
         }
         in = out;
     }
-    void *planes[3];
-    int strides[3];
-    for (int c = 0; c < 3; c++)
+    void *planes[3] = {NULL, NULL, NULL};      /* a semi-planar frame has no plane 2 */
+    int strides[3] = {0, 0, 0};
+    for (int c = 0; c <= out->f.max_plane; c++)
     {
         planes[c]  = out->plane[c].data;
         strides[c] = out->plane[c].stride;

@@ -86,7 +86,7 @@ static int comb_detect_cuda_init(hb_filter_object_t *filter, hb_filter_init_t *i
     hb_buffer_list_clear(&pv->out_list);
 
     const AVPixFmtDescriptor *desc = av_pix_fmt_desc_get(init->pix_fmt);
-    if (desc == NULL)
+    if (desc == NULL || av_pix_fmt_count_planes(init->pix_fmt) < 3)    /* planar YUV only */
     {
         hb_error("comb_detect(cuda): unsupported pixel format %d", init->pix_fmt);
         goto fail;

@@ -86,7 +86,7 @@ static int denoise_cuda_init(hb_filter_object_t *filter, hb_filter_init_t *init)
     int16_t *tab[6] = { NULL, NULL, NULL, NULL, NULL, NULL };
 
     const AVPixFmtDescriptor *desc = av_pix_fmt_desc_get(init->pix_fmt);
-    if (desc == NULL || desc->nb_components < 3)
+    if (desc == NULL || desc->nb_components < 3 || av_pix_fmt_count_planes(init->pix_fmt) < 3)    /* planar YUV only */
     {
         hb_error("denoise(cuda): unsupported pixel format %d", init->pix_fmt);
         goto fail;

@@ -85,9 +85,16 @@ enum AVPixelFormat
     AV_PIX_FMT_YUVA420P    = 33,
     AV_PIX_FMT_YUVA422P    = 78,
     AV_PIX_FMT_YUVA444P    = 79,
+    /* the semi-planar 4:2:0 formats NVDEC decodes into (AVHWFramesContext.sw_format): Y, then one plane of
+     * interleaved Cb/Cr pairs; P010 keeps its 10 bits in the high bits of each 16-bit sample */
+    AV_PIX_FMT_NV12        = 23,
+    AV_PIX_FMT_P010LE      = 158,
+    AV_PIX_FMT_P016LE      = 169,
 };
 #define AV_PIX_FMT_YUV420P10 AV_PIX_FMT_YUV420P10LE
 #define AV_PIX_FMT_YUV420P12 AV_PIX_FMT_YUV420P12LE
+#define AV_PIX_FMT_P010      AV_PIX_FMT_P010LE
+#define AV_PIX_FMT_P016      AV_PIX_FMT_P016LE
 
 /* FFmpeg's enum AVChromaLocation (libavutil/pixfmt.h) */
 enum AVChromaLocation

@@ -30,7 +30,7 @@ size_t hb_harness_frame_bytes(int pix_fmt, int w, int h)
     const AVPixFmtDescriptor *d = av_pix_fmt_desc_get(pix_fmt);
     if (d == NULL) return 0;
     size_t total = 0;
-    int nplanes = d->nb_components;
+    const int nplanes = av_pix_fmt_count_planes(pix_fmt);
     for (int p = 0; p < nplanes; p++)
         total += (size_t)av_image_get_linesize(pix_fmt, w, p) * hb_image_height(pix_fmt, h, p);
     return total;
@@ -357,21 +357,18 @@ static void render_sub_harness_close(hb_filter_object_t *filter)
     filter->private_data = NULL;
 }
 
-static int plane_bps(const hb_buffer_t *b)
-{
-    const AVPixFmtDescriptor *d = av_pix_fmt_desc_get(b->f.fmt);
-    return d->comp[0].depth > 8 ? 2 : 1;
-}
+/* bytes of one row of plane p (FFmpeg's linesize: interleaved Cb/Cr pairs count twice), and per sample position */
+static int row_bytes(const hb_buffer_t *b, int p) { return av_image_get_linesize(b->f.fmt, b->f.width, p); }
+static int sample_bytes(const hb_buffer_t *b, int p) { return row_bytes(b, p) / b->plane[p].width; }
 
 /* a host frame with guard_x spare samples and guard_y spare rows around every plane, filled with GUARD_BYTE: writes
  * outside the picture land in memory the frame owns and can be found afterwards */
 static hb_buffer_t *guarded_copy(const hb_buffer_t *in, int gx, int gy)
 {
-    const int bps = plane_bps(in);
-    int stride[3], size = 0;
-    for (int p = 0; p < 3; p++)
+    int stride[4], size = 0;
+    for (int p = 0; p <= in->f.max_plane; p++)
     {
-        stride[p] = HB_ALIGN((in->plane[p].width + 2 * gx) * bps, 64);
+        stride[p] = HB_ALIGN((in->plane[p].width + 2 * gx) * sample_bytes(in, p), 64);
         size += stride[p] * (in->plane[p].height + 2 * gy);
     }
     hb_buffer_t *b = hb_buffer_init(size);
@@ -380,15 +377,16 @@ static hb_buffer_t *guarded_copy(const hb_buffer_t *in, int gx, int gy)
     b->f = in->f;
     hb_buffer_copy_props(b, in);
     uint8_t *base = b->data;
-    for (int p = 0; p < 3; p++)
+    for (int p = 0; p <= in->f.max_plane; p++)
     {
+        const int sb = sample_bytes(in, p);
         b->plane[p] = in->plane[p];
         b->plane[p].stride = stride[p];
-        b->plane[p].data = base + (size_t)gy * stride[p] + (size_t)gx * bps;
+        b->plane[p].data = base + (size_t)gy * stride[p] + (size_t)gx * sb;
         b->plane[p].size = stride[p] * in->plane[p].height;
         for (int y = 0; y < in->plane[p].height; y++)
             memcpy(b->plane[p].data + (size_t)y * stride[p], in->plane[p].data + (size_t)y * in->plane[p].stride,
-                   (size_t)in->plane[p].width * bps);
+                   (size_t)row_bytes(in, p));
         base += (size_t)stride[p] * (in->plane[p].height + 2 * gy);
     }
     return b;
@@ -397,17 +395,17 @@ static hb_buffer_t *guarded_copy(const hb_buffer_t *in, int gx, int gy)
 /* every byte of the guarded allocation outside the pictures still GUARD_BYTE? */
 static int guard_intact(const hb_buffer_t *b, int gx, int gy)
 {
-    const int bps = plane_bps(b);
-    for (int p = 0; p < 3; p++)
+    for (int p = 0; p <= b->f.max_plane; p++)
     {
-        const int stride = b->plane[p].stride, w = b->plane[p].width * bps, h = b->plane[p].height;
-        const uint8_t *row0 = b->plane[p].data - (size_t)gy * stride - (size_t)gx * bps;
+        const int sb = sample_bytes(b, p);
+        const int stride = b->plane[p].stride, w = row_bytes(b, p), h = b->plane[p].height;
+        const uint8_t *row0 = b->plane[p].data - (size_t)gy * stride - (size_t)gx * sb;
         for (int y = 0; y < h + 2 * gy; y++)
         {
             const uint8_t *r = row0 + (size_t)y * stride;
             const int inside = y >= gy && y < gy + h;
             for (int x = 0; x < stride; x++)
-                if ((!inside || x < gx * bps || x >= gx * bps + w) && r[x] != GUARD_BYTE) return 0;
+                if ((!inside || x < gx * sb || x >= gx * sb + w) && r[x] != GUARD_BYTE) return 0;
         }
     }
     return 1;
@@ -421,11 +419,10 @@ static hb_buffer_t *unguarded_copy(const hb_buffer_t *g)
     b->f = g->f;
     b->f.max_plane = tmp.f.max_plane;
     hb_buffer_copy_props(b, g);
-    const int bps = plane_bps(g);
-    for (int p = 0; p < 3; p++)
+    for (int p = 0; p <= b->f.max_plane; p++)
         for (int y = 0; y < b->plane[p].height; y++)
             memcpy(b->plane[p].data + (size_t)y * b->plane[p].stride, g->plane[p].data + (size_t)y * g->plane[p].stride,
-                   (size_t)b->plane[p].width * bps);
+                   (size_t)row_bytes(b, p));
     return b;
 }
 

@@ -40,6 +40,12 @@ static const AVPixFmtDescriptor desc_yuv420p16  = DESC("yuv420p16le", 1, 1, 16, 
 static const AVPixFmtDescriptor desc_yuva420p   = DESC_A("yuva420p", 1, 1);
 static const AVPixFmtDescriptor desc_yuva422p   = DESC_A("yuva422p", 1, 0);
 static const AVPixFmtDescriptor desc_yuva444p   = DESC_A("yuva444p", 0, 0);
+/* libavutil/pixdesc.c: Cb and Cr share plane 1, interleaved (step = one Cb/Cr pair, Cr one sample after Cb) */
+#define DESC_SEMI(nm, bytes, sh, d) \
+    { nm, 3, 1, 1, 0, { {0, bytes, 0, sh, d}, {1, 2 * (bytes), 0, sh, d}, {1, 2 * (bytes), bytes, sh, d}, {0, 0, 0, 0, 0} } }
+static const AVPixFmtDescriptor desc_nv12       = DESC_SEMI("nv12",    1, 0,  8);
+static const AVPixFmtDescriptor desc_p010       = DESC_SEMI("p010le",  2, 6, 10);
+static const AVPixFmtDescriptor desc_p016       = DESC_SEMI("p016le",  2, 0, 16);
 
 const AVPixFmtDescriptor *av_pix_fmt_desc_get(int pix_fmt)
 {
@@ -57,6 +63,9 @@ const AVPixFmtDescriptor *av_pix_fmt_desc_get(int pix_fmt)
         case AV_PIX_FMT_YUVA420P:    return &desc_yuva420p;
         case AV_PIX_FMT_YUVA422P:    return &desc_yuva422p;
         case AV_PIX_FMT_YUVA444P:    return &desc_yuva444p;
+        case AV_PIX_FMT_NV12:        return &desc_nv12;
+        case AV_PIX_FMT_P010LE:      return &desc_p010;
+        case AV_PIX_FMT_P016LE:      return &desc_p016;
         default:                     return NULL;
     }
 }
@@ -98,6 +107,18 @@ __attribute__((weak)) void hb_compute_chroma_smoothing_coefficient(uint32_t chro
 int av_image_get_linesize(int pix_fmt, int width, int plane)
 {
     const AVPixFmtDescriptor *d = av_pix_fmt_desc_get(pix_fmt);
+    if (d != NULL && d->nb_components == 3 && d->comp[1].plane == d->comp[2].plane)
+    {
+        /* semi-planar (libavutil/imgutils.c): the largest step of the plane's components times the plane's width in
+         * samples; 0 for a plane the format does not have */
+        if (plane < 0 || plane > 3)
+            return -1;
+        int step = 0;
+        for (int c = 0; c < d->nb_components; c++)
+            if (d->comp[c].plane == plane && d->comp[c].step > step)
+                step = d->comp[c].step;
+        return step * (plane == 1 || plane == 2 ? -((-width) >> d->log2_chroma_w) : width);
+    }
     if (d == NULL || plane < 0 || plane >= d->nb_components)
         return -1;
     int w = width;

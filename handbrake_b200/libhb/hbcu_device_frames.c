@@ -78,27 +78,35 @@ hbcu_frame_t *hbcu_buffer_frame(const hb_buffer_t *b)
     return (b != NULL && b->storage_type == HBCU_DEVICE) ? (hbcu_frame_t *)b->storage : NULL;
 }
 
-hb_buffer_t *hbcu_device_frame_buffer_init(int pix_fmt, int width, int height, int device)
+/* planes of a YUV frame as a device frame has them: 3, or 2 for a semi-planar format (NV12, P010, P016), whose
+ * absent third plane is 0 rows of 0 bytes; row bytes are FFmpeg's linesizes (a row of Cb/Cr pairs is twice as long) */
+static int frame_planes(int pix_fmt)
 {
     const AVPixFmtDescriptor *desc = av_pix_fmt_desc_get(pix_fmt);
-    if (desc == NULL || desc->nb_components < 3) return NULL;
+    if (desc == NULL || desc->nb_components < 3) return 0;
+    return av_pix_fmt_count_planes(pix_fmt) == 2 ? 2 : 3;
+}
+
+hb_buffer_t *hbcu_device_frame_buffer_init(int pix_fmt, int width, int height, int device)
+{
+    const int nplanes = frame_planes(pix_fmt);
+    if (nplanes == 0) return NULL;
     install_hooks();
     hb_buffer_t *b = hb_buffer_init(0);
     if (b == NULL) return NULL;
-    b->f.max_plane = 2;
+    b->f.max_plane = nplanes - 1;
     b->s.type      = FRAME_BUF;
     b->f.width     = width;
     b->f.height    = height;
     b->f.fmt       = pix_fmt;
-    const int bps = desc->comp[0].depth > 8 ? 2 : 1;
-    int row_bytes[3], rows[3], strides[3];
-    for (int p = 0; p < 3; p++)
+    int row_bytes[3] = {0, 0, 0}, rows[3] = {0, 0, 0}, strides[3] = {0, 0, 0};
+    for (int p = 0; p < nplanes; p++)
     {
         b->plane[p].stride = hb_image_stride(pix_fmt, width, p);
         b->plane[p].width  = hb_image_width(pix_fmt, width, p);
         b->plane[p].height = hb_image_height(pix_fmt, height, p);
         b->plane[p].size   = b->plane[p].stride * b->plane[p].height;
-        row_bytes[p] = b->plane[p].width * bps;
+        row_bytes[p] = av_image_get_linesize(pix_fmt, width, p);
         rows[p]      = b->plane[p].height;
         strides[p]   = b->plane[p].stride;
         b->size     += b->plane[p].size;
@@ -110,7 +118,7 @@ hb_buffer_t *hbcu_device_frame_buffer_init(int pix_fmt, int width, int height, i
         hb_buffer_close(&b);
         return NULL;
     }
-    for (int p = 0; p < 3; p++) b->plane[p].data = hbcu_frame_plane(f, p);
+    for (int p = 0; p < nplanes; p++) b->plane[p].data = hbcu_frame_plane(f, p);
     b->storage_type = HBCU_DEVICE;
     b->storage = f;
     return b;
@@ -119,35 +127,38 @@ hb_buffer_t *hbcu_device_frame_buffer_init(int pix_fmt, int width, int height, i
 /* The decoder end of a zero-copy chain (SURVEY.md 8 f4): an AVFrame of AV_PIX_FMT_CUDA -- data[i] device pointers,
  * linesize[i], the frames context's device and stream -- becomes an HBCU_DEVICE hb_buffer_t without a copy
  * (hwaccel.c:15-60 is where libhb receives such frames; nvenc_common.c:329-336 where the encoder asks for them).
+ * For NVDEC's semi-planar sw_format (NV12, P010, P016) only data[0..1] / linesize[0..1] are read.
  * `release(opaque)` is the caller's av_frame_free: it runs when the buffer is closed and the last device reader is done. */
 hb_buffer_t *hbcu_wrap_cuda_frame(int pix_fmt, int width, int height, int device, void *const data[3], const int linesize[3],
                                   size_t readable_tail_bytes, void *cuda_stream, void (*release)(void *), void *opaque)
 {
-    const AVPixFmtDescriptor *desc = av_pix_fmt_desc_get(pix_fmt);
-    if (desc == NULL || desc->nb_components < 3) return NULL;
+    const int nplanes = frame_planes(pix_fmt);
+    if (nplanes == 0) return NULL;
     install_hooks();
     hb_buffer_t *b = hb_buffer_init(0);
     if (b == NULL) return NULL;
-    b->f.max_plane = 2;
+    b->f.max_plane = nplanes - 1;
     b->s.type      = FRAME_BUF;
     b->f.width     = width;
     b->f.height    = height;
     b->f.fmt       = pix_fmt;
-    const int bps = desc->comp[0].depth > 8 ? 2 : 1;
-    int row_bytes[3], rows[3];
-    for (int p = 0; p < 3; p++)
+    void *planes[3] = {NULL, NULL, NULL};
+    int row_bytes[3] = {0, 0, 0}, rows[3] = {0, 0, 0}, strides[3] = {0, 0, 0};
+    for (int p = 0; p < nplanes; p++)
     {
         b->plane[p].stride = linesize[p];
         b->plane[p].width  = hb_image_width(pix_fmt, width, p);
         b->plane[p].height = hb_image_height(pix_fmt, height, p);
         b->plane[p].size   = b->plane[p].stride * b->plane[p].height;
         b->plane[p].data   = data[p];
-        row_bytes[p] = b->plane[p].width * bps;
+        planes[p]    = data[p];
+        strides[p]   = linesize[p];
+        row_bytes[p] = av_image_get_linesize(pix_fmt, width, p);
         rows[p]      = b->plane[p].height;
         b->size     += b->plane[p].size;
     }
     hbcu_frame_t *f = NULL;
-    if (hbcu_frame_wrap(&f, device, data, row_bytes, rows, linesize, readable_tail_bytes, cuda_stream, release, opaque) != 0)
+    if (hbcu_frame_wrap(&f, device, planes, row_bytes, rows, strides, readable_tail_bytes, cuda_stream, release, opaque) != 0)
     {
         hb_error("hbcu: wrapped device frame: %s", hbcu_last_error());
         hb_buffer_close(&b);
@@ -262,10 +273,10 @@ static void surface_return(void *opaque)
 /* test hook: the uploaded frame plays a decoder-owned surface; what goes downstream is a wrapper around its planes */
 static hb_buffer_t *as_decoder_surface(hb_filter_private_t *pv, hb_buffer_t *surface)
 {
-    void *data[3];
-    int linesize[3];
+    void *data[3] = {NULL, NULL, NULL};
+    int linesize[3] = {0, 0, 0};
     if (hbcu_xfer_wait(pv->x, pv->pending[pv->head].ticket) != 0) return NULL;      /* the "decode" is complete */
-    for (int c = 0; c < 3; c++)
+    for (int c = 0; c <= surface->f.max_plane; c++)
     {
         data[c]     = surface->plane[c].data;
         linesize[c] = surface->plane[c].stride;
@@ -353,9 +364,9 @@ static int xfer_work(hb_filter_object_t *filter, hb_buffer_t **buf_in, hb_buffer
         out->f.chroma_location = in->f.chroma_location;
         hb_buffer_copy_props(out, in);
         hb_buffer_t *host = pv->download ? out : in;
-        void *planes[3];
-        int strides[3];
-        for (int c = 0; c < 3; c++)
+        void *planes[3] = {NULL, NULL, NULL};
+        int strides[3] = {0, 0, 0};
+        for (int c = 0; c <= host->f.max_plane; c++)
         {
             planes[c]  = host->plane[c].data;
             strides[c] = host->plane[c].stride;

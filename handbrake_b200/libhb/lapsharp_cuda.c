@@ -72,7 +72,7 @@ static int lapsharp_cuda_init(hb_filter_object_t *filter, hb_filter_init_t *init
     pv->input = *init;
 
     const AVPixFmtDescriptor *desc = av_pix_fmt_desc_get(init->pix_fmt);
-    if (desc == NULL || desc->nb_components < 3)
+    if (desc == NULL || desc->nb_components < 3 || av_pix_fmt_count_planes(init->pix_fmt) < 3)    /* planar YUV only */
     {
         hb_error("lapsharp(cuda): unsupported pixel format %d", init->pix_fmt);
         goto fail;

@@ -163,7 +163,7 @@ int hb_nlmeans_cuda_build_config(const hb_dict_t *dict, int pix_fmt, int width, 
     int threads = -1, max_frames = 0;
 
     const AVPixFmtDescriptor *desc = av_pix_fmt_desc_get(pix_fmt);
-    if (desc == NULL || desc->nb_components < 3)
+    if (desc == NULL || desc->nb_components < 3 || av_pix_fmt_count_planes(pix_fmt) < 3)    /* planar YUV only */
     {
         hb_error("nlmeans(cuda): unsupported pixel format %d", pix_fmt);
         return -1;

@@ -98,6 +98,14 @@ static int metric_init(hb_filter_private_t *pv, hb_filter_init_t *init)
         hb_error("vfr(cuda): unsupported pixel format %d", init->pix_fmt);
         return -1;
     }
+    /* P010 / P016 keep their samples in the high bits: the reference indexes its (1 << depth)-entry table with them
+     * (motion_metric.c:240-251, 285-291), past its end for P010.  Above 8 bits a semi-planar frame is for mode 0 only;
+     * NV12 is fine, the metric reads plane 0 */
+    if (av_pix_fmt_count_planes(init->pix_fmt) == 2 && desc->comp[0].depth > 8)
+    {
+        hb_error("vfr(cuda): the motion metric does not take %s frames; only mode 0 (variable frame rate) does", desc->name);
+        return -1;
+    }
     const int depth = desc->comp[0].depth, max_value = (1 << depth) - 1;
     unsigned *lut = malloc(sizeof(unsigned) * (max_value + 1));
     if (lut == NULL)

@@ -10,6 +10,10 @@ import numpy as np
 PIX_FMT_YUV420P = 0        # values follow the shim's enum AVPixelFormat
 PIX_FMT_YUV420P10 = 62
 PIX_FMT_YUV420P12 = 123
+# semi-planar 4:2:0 (what NVDEC decodes into): Y, then one plane of Cb/Cr pairs; P010 keeps 10 bits in the high bits
+PIX_FMT_NV12 = 23
+PIX_FMT_P010 = 158
+PIX_FMT_P016 = 169
 
 PIC_FLAG_TOP_FIELD_FIRST = 0x0008
 PIC_FLAG_PROGRESSIVE_FRAME = 0x0010

@@ -63,6 +63,9 @@ uint64_t     hbcu_kernel_launches(void);
 /*   back at the given strides (use hb_image_stride: the layout of a STANDARD  */
 /*   hb_buffer_t).  Frames are pooled; release never blocks -- two CUDA events */
 /*   per frame (producer done / readers done) order the streams that touch it. */
+/*   A semi-planar frame (NV12, P010, P016: Y, then interleaved Cb/Cr) has two */
+/*   planes: its third plane is given as rows == 0, row_bytes == 0 (and a NULL */
+/*   pointer to hbcu_frame_wrap); hbcu_frame_plane(f, 2) is then NULL.          */
 /* ------------------------------------------------------------------------- */
 typedef struct hbcu_frame_s hbcu_frame_t;
 int    hbcu_frame_alloc(hbcu_frame_t **f, int device, const int row_bytes[3], const int rows[3], const int strides[3]);
@@ -457,8 +460,10 @@ int  hbcu_detelecine_elapsed_ms(hbcu_detelecine_t *h, float *ms);
 
 /* ------------------------------------------------------------------------- */
 /* blend        replaces the overlay compositing of libhb/blend.c (blend8on8,   */
-/*              blend8on1x, blend_subsample_8on8, blend_subsample_8on1x):        */
-/*              burned-in subtitles (rendersub.c) on planar YUV frames           */
+/*              blend8on1x, blend_subsample_8on8, blend_subsample_8on1x and the  */
+/*              semi-planar blend8onbi8, blend8onbi1x, blend_subsample_8onbi8,   */
+/*              blend_subsample_8onbi1x): burned-in subtitles (rendersub.c) on   */
+/*              planar YUV and on NV12 / P010 / P016 frames                      */
 /* ------------------------------------------------------------------------- */
 /* One handle per frame geometry.  Overlays are 8-bit YUVA with the frame's chroma subsampling (the plain path of
  * blend.c) or YUVA 4:4:4 on a subsampled frame (the subsample path: every chroma sample takes the chroma-location
@@ -470,6 +475,9 @@ typedef struct hbcu_blend_config_s
     int overlay_shift_w, overlay_shift_h;/* overlay chroma subsampling: the frame's, or (0,0) for YUVA 4:4:4 */
     int device;
     uint32_t chroma_coeffs[2][4];        /* hb_compute_chroma_smoothing_coefficient() of the frame's format and chroma location */
+    int interleaved_chroma;              /* 0: planes Y, Cb, Cr; 1: semi-planar 4:2:0 (NV12, P010, P016), plane 1 holds Cb/Cr
+                                          * pairs and plane 2 is absent (NULL, stride 0).  Semi-planar frames follow blend.c's
+                                          * *bi* functions: above 8 bits overlay samples are scaled by << 8, not << (depth - 8) */
 } hbcu_blend_config_t;
 
 typedef struct hbcu_blend_overlay_s

@@ -4,6 +4,9 @@ Workloads (what libhb's subtitle renderer hands hb_blend_cuda):
   pgs  4K yuv420p10, two 1600x120 YUVA 4:4:4 overlays (subsample path), list unchanged in steady state
   ssa  4K yuv420p10, one 3840x400 YUVA 4:2:0 band (plain path), list unchanged in steady state
   vob  1080p yuv420p, one full-frame YUVA 4:4:4 overlay, a new list every frame (an upload per frame)
+and, for a hardware-decoded job, the semi-planar formats NVDEC decodes into next to their planar pairs (same bytes):
+  pgs  4K P010 against 4K yuv420p10 above
+  ssa  1080p NV12 against 1080p yuv420p, one 1920x200 YUVA 4:2:0 band (plain path)
 
 device ms/frame  CUDA events around K device-frame blends (hbcu_blend_mark / elapsed_ms): the device-to-device copy of
                  the frame plus the one blend launch; `2F share` is the time 2 x frame bytes take at 3.35 TB/s (H100 HBM3
@@ -38,7 +41,7 @@ HBM_PEAK = 3.35e12
 class Config(C.Structure):
     _fields_ = [("width", C.c_int), ("height", C.c_int), ("depth", C.c_int), ("chroma_shift_w", C.c_int),
                 ("chroma_shift_h", C.c_int), ("overlay_shift_w", C.c_int), ("overlay_shift_h", C.c_int),
-                ("device", C.c_int), ("chroma_coeffs", C.c_uint32 * 8)]
+                ("device", C.c_int), ("chroma_coeffs", C.c_uint32 * 8), ("interleaved_chroma", C.c_int)]
 
 
 class Overlay(C.Structure):
@@ -47,10 +50,13 @@ class Overlay(C.Structure):
 
 
 WORKLOADS = {
-    # name: (frame w, h, depth, pix_fmt, overlay shifts, overlays (x, y, w, h), changed every frame)
-    "4k_pgs_420p10": (3840, 2160, 10, 62, (0, 0), [(1120, 1880, 1600, 120), (1120, 2010, 1600, 120)], False),
-    "4k_ssa_band_420p10": (3840, 2160, 10, 62, (1, 1), [(0, 1700, 3840, 400)], False),
-    "1080p_vobsub_fullframe_420p": (1920, 1080, 8, 0, (0, 0), [(0, 0, 1920, 1080)], True),
+    # name: (frame w, h, depth, pix_fmt, overlay shifts, overlays (x, y, w, h), changed every frame, semi-planar)
+    "4k_pgs_420p10": (3840, 2160, 10, 62, (0, 0), [(1120, 1880, 1600, 120), (1120, 2010, 1600, 120)], False, False),
+    "4k_pgs_p010": (3840, 2160, 10, 158, (0, 0), [(1120, 1880, 1600, 120), (1120, 2010, 1600, 120)], False, True),
+    "4k_ssa_band_420p10": (3840, 2160, 10, 62, (1, 1), [(0, 1700, 3840, 400)], False, False),
+    "1080p_ssa_band_420p": (1920, 1080, 8, 0, (1, 1), [(0, 850, 1920, 200)], False, False),
+    "1080p_ssa_band_nv12": (1920, 1080, 8, 23, (1, 1), [(0, 850, 1920, 200)], False, True),
+    "1080p_vobsub_fullframe_420p": (1920, 1080, 8, 0, (0, 0), [(0, 0, 1920, 1080)], True, False),
 }
 
 
@@ -82,9 +88,10 @@ def make_overlays(shifts, rects, seed):
 
 
 def bench_gpu(lib, name, steps, warmup):
-    w, h, depth, pix, osh, rects, changed = WORKLOADS[name]
+    w, h, depth, pix, osh, rects, changed, semi = WORKLOADS[name]
     sw, sh = 1, 1
     cfg = Config(w, h, depth, sw, sh, osh[0], osh[1], 0)
+    cfg.interleaved_chroma = int(semi)
     for i, v in enumerate([18, 18, 6, 2, 18, 18, 6, 2]):      # center chroma location, 4:2:0
         cfg.chroma_coeffs[i] = v
     hnd = C.c_void_p()
@@ -92,8 +99,9 @@ def bench_gpu(lib, name, steps, warmup):
         raise RuntimeError(lib.hbcu_last_error().decode())
     bps = 2 if depth > 8 else 1
     cw, ch = (w + 1) // 2, (h + 1) // 2
-    row_bytes = (C.c_int * 3)(w * bps, cw * bps, cw * bps)
-    rows = (C.c_int * 3)(h, ch, ch)
+    # a semi-planar frame: one plane of Cb/Cr pairs, the third plane absent (0 rows of 0 bytes)
+    row_bytes = (C.c_int * 3)(w * bps, 2 * cw * bps, 0) if semi else (C.c_int * 3)(w * bps, cw * bps, cw * bps)
+    rows = (C.c_int * 3)(h, ch, 0) if semi else (C.c_int * 3)(h, ch, ch)
     strides = (C.c_int * 3)(*[(rb + 63) // 64 * 64 for rb in row_bytes])
     frame_bytes = sum(strides[p] * rows[p] for p in range(3))
     fin = C.c_void_p()
@@ -132,7 +140,7 @@ def bench_cpu(name, frames_n=8):
     if not ref_so.exists():
         return None
     from handbrake_b200.hblib import FilterLib, RENDER_SUB
-    w, h, depth, pix, osh, rects, changed = WORKLOADS[name]
+    w, h, depth, pix, osh, rects, changed, _ = WORKLOADS[name]
     lib = FilterLib(ref_so)
     bps = 2 if depth > 8 else 1
     fb = (w * h + 2 * ((w + 1) // 2) * ((h + 1) // 2)) * bps
