@@ -1490,6 +1490,7 @@ struct hbcu_nlmeans_s
     std::vector<CUtensorMap> maps3f;      // same planes, box height of nlmeans_v3f_kernel's tile (v3_fused only)
     int v3_nw, v3_rs;                     // v3 kernel shape (warps, rows per warp); v3_nw == 0: off
     bool v3_fused;                        // range 3 with nf <= 2 runs nlmeans_v3f_kernel (HBCU_NLMEANS_V3_FUSED=0: off)
+    int v3f_rs;                           // its rows per warp (v3f_pick_rs), the box height of maps3f
     float *d_exptable;                    // 3 x 128
     unsigned *d_range_flag;               // sticky: a 16-bit plane held a sample above kFast16Max (see nlmeans_fast16_kernel)
     cudaStream_t s_h2d, s_pad, s_compute, s_d2h;   // s_compute = s_comp[frame index & (n_comp - 1)] of the launch being queued
@@ -1713,15 +1714,32 @@ int launch_v3_pre(FusedParams &fp, cudaStream_t st)
 // (NH = 4) needs 8 warps (its 9-row history does not fit 168 registers).
 struct V3Shape { int nw, rs; };
 constexpr V3Shape kV3Default = { 12, 10 };
-// nlmeans_v3f_kernel keeps no accumulators in shared memory, so its tile can be taller.  12 x 20 (a 240-row tile) was
-// measured against 12 x 30 (H100 80GB HBM3, 700 W power limit): 30-row strips are 3.5 % faster at 4K but 15 % slower
-// at 1080p, whose 360-row tiles leave SMs idle.  168 registers, no spills.
+// nlmeans_v3f_kernel keeps no accumulators in shared memory, so its tile can be taller.  It is built in two shapes,
+// 12 x 20 (a 240-row tile) and 12 x 30 (360 rows), and a handle picks one from its frame size (v3f_pick_rs).  A taller
+// strip spreads its warm-up (2 NH + 1 patch rows per frame) and the CTA's set-up over more output rows, but a frame has
+// a third fewer CTAs.  168 registers, no spills.
 constexpr V3Shape kV3Fused = { 12, 20 };
+constexpr V3Shape kV3FusedTall = { 12, 30 };
 
-template <int NH>
+// CTAs of one frame (all three planes) in nlmeans_v3f_kernel at strips of rs rows
+int v3f_tiles(const PlaneGeom *g, int rs)
+{
+    int n = 0;
+    for (int pl = 0; pl < 3; pl++) n += (g[pl].w + kTileW - 1) / kTileW * ((g[pl].h + kV3Fused.nw * rs - 1) / (kV3Fused.nw * rs));
+    return n;
+}
+
+// The tall shape when its CTAs still give every SM at least one per frame: on an H100 SXM (132 SMs) a 4K 4:2:0 frame
+// has 270 tall CTAs (420 short), a 1080p frame 77 (123 short) -- there the tall shape would leave 55 SMs without work.
+int v3f_pick_rs(const PlaneGeom *g, int sms)
+{
+    return v3f_tiles(g, kV3FusedTall.rs) >= sms ? kV3FusedTall.rs : kV3Fused.rs;
+}
+
+template <int NH, int RS>
 int launch_v3f(FusedParams &fp, cudaStream_t st)
 {
-    constexpr int NW = kV3Fused.nw, RS = kV3Fused.rs;
+    constexpr int NW = kV3Fused.nw;
     using L = V3FusedLayout<NW, RS>;
     // function attributes live in the device's context: one flag per device
     static bool configured_on[kMaxDevices] = {};
@@ -1763,15 +1781,22 @@ bool v3f_ok(const hbcu_nlmeans_s *h, const KernelParams *kps, const bool *active
     return any;
 }
 
-int launch_v3f_nh(FusedParams &fp, cudaStream_t st)
+int launch_v3f_nh(int rs, FusedParams &fp, cudaStream_t st)
 {
-    switch (fp.k[0].n_half)
+    static_assert(kV3Fused.nw == kV3FusedTall.nw, "one warp count");
+    constexpr int S = kV3Fused.rs, T = kV3FusedTall.rs;
+    const int nh = fp.k[0].n_half;
+    if (rs == T)
     {
-        case 1: return launch_v3f<1>(fp, st);
-        case 2: return launch_v3f<2>(fp, st);
-        case 3: return launch_v3f<3>(fp, st);
-        default: return 1;
+        if (nh == 1) return launch_v3f<1, T>(fp, st);
+        if (nh == 2) return launch_v3f<2, T>(fp, st);
+        if (nh == 3) return launch_v3f<3, T>(fp, st);
+        return 1;
     }
+    if (nh == 1) return launch_v3f<1, S>(fp, st);
+    if (nh == 2) return launch_v3f<2, S>(fp, st);
+    if (nh == 3) return launch_v3f<3, S>(fp, st);
+    return 1;
 }
 
 // rows of one TMA box of the v3 tile: V3Layout::kBoxRows restated for a run-time shape (the kernel's expect-tx byte
@@ -1961,7 +1986,7 @@ int launch_plane(hbcu_nlmeans_s *h, const KernelParams &kp, const int *slots, in
             const bool v3 = v3_pick(h, kp.n_half, &vs);
             const bool v3f = v3 && v3f_ok(h, &kp, nullptr, 1);
             for (int f = 0; f < kp.nf; f++) fp.maps[0][f] = v3f ? h->maps3f[slots[f] * 3 + plane] : v3 ? h->maps3[slots[f] * 3 + plane] : tp.maps[f];
-            rc = v3f ? launch_v3f_nh(fp, h->s_compute) : v3 ? launch_v3_nh(vs.nw, vs.rs, fp, h->s_compute) : launch_fast8_nh(fp, h->s_compute);
+            rc = v3f ? launch_v3f_nh(h->v3f_rs, fp, h->s_compute) : v3 ? launch_v3_nh(vs.nw, vs.rs, fp, h->s_compute) : launch_fast8_nh(fp, h->s_compute);
         }
         else
             rc = h->bps == 1 ? launch_tiled_nh<uint8_t, kTH8>(tp, h->s_compute) : launch_tiled_nh<uint16_t, kTH16>(tp, h->s_compute);
@@ -2174,7 +2199,7 @@ int run_filter(hbcu_nlmeans_s *h, int64_t index, int navail, int oslot, void *co
             for (int f = 0; f < kps[pl].nf; f++) fp.maps[fp.nplanes][f] = (v3f ? h->maps3f : v3 ? h->maps3 : h->maps)[slots[pl][f] * 3 + pl];
             fp.nplanes++;
         }
-        const int rc8 = v3f ? launch_v3f_nh(fp, h->s_compute) : v3 ? launch_v3_nh(vs.nw, vs.rs, fp, h->s_compute) : launch_fast8_nh(fp, h->s_compute);
+        const int rc8 = v3f ? launch_v3f_nh(h->v3f_rs, fp, h->s_compute) : v3 ? launch_v3_nh(vs.nw, vs.rs, fp, h->s_compute) : launch_fast8_nh(fp, h->s_compute);
         if (rc8 < 0) { set_error("nlmeans: fused launch failed"); return -1; }
         if (rc8 == 0)
         {
@@ -2315,6 +2340,12 @@ int hbcu_nlmeans_create(hbcu_nlmeans_t **out, const hbcu_nlmeans_config_t *cfg)
             return -1;                                                                                    \
         }                                                                                                 \
     } while (0)
+    int sms = 0;
+    CK(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, cfg->device));
+    h->v3f_rs = v3f_pick_rs(h->g, sms);
+    // HBCU_NLMEANS_V3F_RS=20|30: one shape regardless of frame size (test hook: small frames reach the tall shape)
+    if (const char *e = getenv("HBCU_NLMEANS_V3F_RS"))
+        if (atoi(e) == kV3Fused.rs || atoi(e) == kV3FusedTall.rs) h->v3f_rs = atoi(e);
     // The NLMeans kernel fills every SM (one CTA takes the whole register file); the small border kernels
     // of the upload stream must not queue behind a whole frame of it, or the upload -> kernel chain stalls:
     // give the upload stream the highest priority so its CTAs are placed as soon as any SM frees up.
@@ -2405,7 +2436,7 @@ int hbcu_nlmeans_create(hbcu_nlmeans_t **out, const hbcu_nlmeans_config_t *cfg)
             if (h->v3_fused &&
                 hbcu::encode_tensor_map_2d(&h->maps3f[s * 3 + pl], h->bps, h->ring_mem[s * 3 + pl], (uint64_t)h->g[pl].bw,
                                            (uint64_t)h->g[pl].bh, (uint64_t)h->g[pl].bpitch * h->bps, kTilePW,
-                                           v3_box_rows(kV3Fused.nw, kV3Fused.rs)) != 0)
+                                           v3_box_rows(kV3Fused.nw, h->v3f_rs)) != 0)
             {
                 hbcu_nlmeans_destroy(h);
                 return -1;
