@@ -1714,12 +1714,14 @@ int launch_v3_pre(FusedParams &fp, cudaStream_t st)
 // (NH = 4) needs 8 warps (its 9-row history does not fit 168 registers).
 struct V3Shape { int nw, rs; };
 constexpr V3Shape kV3Default = { 12, 10 };
-// nlmeans_v3f_kernel keeps no accumulators in shared memory, so its tile can be taller.  It is built in two shapes,
-// 12 x 20 (a 240-row tile) and 12 x 30 (360 rows), and a handle picks one from its frame size (v3f_pick_rs).  A taller
-// strip spreads its warm-up (2 NH + 1 patch rows per frame) and the CTA's set-up over more output rows, but a frame has
-// a third fewer CTAs.  168 registers, no spills.
+// nlmeans_v3f_kernel keeps no accumulators in shared memory, so its tile can be taller.  It is built in three shapes,
+// 12 x 20 (a 240-row tile), 12 x 30 (360 rows) and 12 x 45 (540 rows), and a handle picks one from its frame size
+// (v3f_pick_rs).  A taller strip spreads its warm-up (2 NH + 1 patch rows per frame) and the CTA's set-up over more
+// output rows, but a frame has fewer CTAs.  168 registers, no spills.
 constexpr V3Shape kV3Fused = { 12, 20 };
 constexpr V3Shape kV3FusedTall = { 12, 30 };
+constexpr V3Shape kV3FusedTaller = { 12, 45 };
+constexpr int kV3FusedWarmRows = 7;      // 2 NH + 1 at patch 7: the warm-up rows the shape rule charges each strip
 
 // CTAs of one frame (all three planes) in nlmeans_v3f_kernel at strips of rs rows
 int v3f_tiles(const PlaneGeom *g, int rs)
@@ -1729,10 +1731,17 @@ int v3f_tiles(const PlaneGeom *g, int rs)
     return n;
 }
 
-// The tall shape when its CTAs still give every SM at least one per frame: on an H100 SXM (132 SMs) a 4K 4:2:0 frame
-// has 270 tall CTAs (420 short), a 1080p frame 77 (123 short) -- there the tall shape would leave 55 SMs without work.
+// modelled SM-rows of one frame at strips of rs rows: every strip marches its rs rows after its warm-up, a partial tile
+// costs a whole one
+long v3f_sm_rows(const PlaneGeom *g, int rs) { return (long)v3f_tiles(g, rs) * (rs + kV3FusedWarmRows); }
+
+// A taller shape only when its CTAs still give every SM at least one per frame; of the two tall shapes the one with the
+// fewer modelled SM-rows (a frame with at least one 45-row CTA per SM has at least one 30-row CTA per SM too).  On an
+// H100 SXM (132 SMs) a 4K 4:2:0 frame has 180 CTAs at 45 rows (270 at 30, 420 at 20) and takes 45; a 1080p frame has
+// 46 (77, 123) and keeps 20 -- the taller shapes would leave SMs without work.
 int v3f_pick_rs(const PlaneGeom *g, int sms)
 {
+    if (v3f_tiles(g, kV3FusedTaller.rs) >= sms && v3f_sm_rows(g, kV3FusedTaller.rs) < v3f_sm_rows(g, kV3FusedTall.rs)) return kV3FusedTaller.rs;
     return v3f_tiles(g, kV3FusedTall.rs) >= sms ? kV3FusedTall.rs : kV3Fused.rs;
 }
 
@@ -1781,29 +1790,29 @@ bool v3f_ok(const hbcu_nlmeans_s *h, const KernelParams *kps, const bool *active
     return any;
 }
 
+template <int RS>
+int launch_v3f_rs(FusedParams &fp, cudaStream_t st)
+{
+    const int nh = fp.k[0].n_half;
+    if (nh == 1) return launch_v3f<1, RS>(fp, st);
+    if (nh == 2) return launch_v3f<2, RS>(fp, st);
+    if (nh == 3) return launch_v3f<3, RS>(fp, st);
+    return 1;
+}
+
 int launch_v3f_nh(int rs, FusedParams &fp, cudaStream_t st)
 {
-    static_assert(kV3Fused.nw == kV3FusedTall.nw, "one warp count");
-    constexpr int S = kV3Fused.rs, T = kV3FusedTall.rs;
-    const int nh = fp.k[0].n_half;
-    if (rs == T)
-    {
-        if (nh == 1) return launch_v3f<1, T>(fp, st);
-        if (nh == 2) return launch_v3f<2, T>(fp, st);
-        if (nh == 3) return launch_v3f<3, T>(fp, st);
-        return 1;
-    }
-    if (nh == 1) return launch_v3f<1, S>(fp, st);
-    if (nh == 2) return launch_v3f<2, S>(fp, st);
-    if (nh == 3) return launch_v3f<3, S>(fp, st);
-    return 1;
+    static_assert(kV3Fused.nw == kV3FusedTall.nw && kV3Fused.nw == kV3FusedTaller.nw, "one warp count");
+    if (rs == kV3FusedTaller.rs) return launch_v3f_rs<kV3FusedTaller.rs>(fp, st);
+    if (rs == kV3FusedTall.rs) return launch_v3f_rs<kV3FusedTall.rs>(fp, st);
+    return launch_v3f_rs<kV3Fused.rs>(fp, st);
 }
 
 // rows of one TMA box of the v3 tile: V3Layout::kBoxRows restated for a run-time shape (the kernel's expect-tx byte
 // count and the tensor map must agree)
 int v3_box_rows(int nw, int rs)
 {
-    const int rows = nw * rs + 2 * kHalo, loads = rows > 256 ? 2 : 1;
+    const int rows = nw * rs + 2 * kHalo, loads = (rows + 255) / 256;
     return ((rows + loads - 1) / loads + 3) / 4 * 4;
 }
 
@@ -2343,9 +2352,9 @@ int hbcu_nlmeans_create(hbcu_nlmeans_t **out, const hbcu_nlmeans_config_t *cfg)
     int sms = 0;
     CK(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, cfg->device));
     h->v3f_rs = v3f_pick_rs(h->g, sms);
-    // HBCU_NLMEANS_V3F_RS=20|30: one shape regardless of frame size (test hook: small frames reach the tall shape)
+    // HBCU_NLMEANS_V3F_RS=20|30|45: one shape regardless of frame size (test hook: small frames reach the tall shapes)
     if (const char *e = getenv("HBCU_NLMEANS_V3F_RS"))
-        if (atoi(e) == kV3Fused.rs || atoi(e) == kV3FusedTall.rs) h->v3f_rs = atoi(e);
+        if (atoi(e) == kV3Fused.rs || atoi(e) == kV3FusedTall.rs || atoi(e) == kV3FusedTaller.rs) h->v3f_rs = atoi(e);
     // The NLMeans kernel fills every SM (one CTA takes the whole register file); the small border kernels
     // of the upload stream must not queue behind a whole frame of it, or the upload -> kernel chain stalls:
     // give the upload stream the highest priority so its CTAs are placed as soon as any SM frees up.

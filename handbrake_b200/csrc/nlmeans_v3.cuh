@@ -1002,7 +1002,7 @@ template <int NW, int RS>
 struct V3FusedLayout
 {
     static constexpr int kTH        = NW * RS;
-    static constexpr int kLoads     = kTH + 2 * kHalo > 256 ? 2 : 1;                     // a TMA box has at most 256 rows
+    static constexpr int kLoads     = (kTH + 2 * kHalo + 255) / 256;                    // a TMA box has at most 256 rows
     static constexpr int kBoxRows   = ((kTH + 2 * kHalo + kLoads - 1) / kLoads + 3) / 4 * 4;
     static constexpr int kTileBytes = kBoxRows * kLoads * kTilePW;
     static constexpr int kLutBytes  = kLutEntries * 32 * (int)sizeof(float);
