@@ -542,7 +542,7 @@ struct TiledParams
     const unsigned *only_if_flag;         // when set: run only if *only_if_flag != 0 (stand-in for the fast 16-bit kernel)
 };
 
-// The fast 8-bit kernel takes up to three planes in ONE launch (tiles of Y, U and V in one grid):
+// The fused-grid kernels take up to three planes in ONE launch (tiles of Y, U and V in one grid):
 // three separate launches end in three partial waves, one launch of all tiles in one.
 struct FusedParams
 {
@@ -659,42 +659,18 @@ __global__ void __launch_bounds__(kThreads, 1) nlmeans_tiled_kernel(const __grid
 }
 
 // ---------------------------------------------------------------------------
-// Fast 8-bit kernel (v2).  Same tiling and the same arithmetic results as the
-// kernel above, re-expressed for the SM's issue rates (CUDA C++ Programming Guide,
-// arithmetic instruction throughput, compute capability 9.0):
-//   * FADD/FMUL/FFMA issue at 4 warp-instr/clk/SM, integer ALU ops (PRMT, LOP3,
-//     IADD3, IMAD) at 2, F2I / I2F.U8 at 0.5.
-//   * For 8-bit pixels every quantity of the patch distance is an integer
-//     below 2^24 (7*7*255^2 = 3.2M), so it is computed in fp32 EXACTLY: the
-//     squared difference is one FFMA into a running prefix sum, the patch-row
-//     sum one FADD, the vertical window two FADDs.  No int->float conversion.
-//   * Pixels are fetched as 32-bit words (conflict-free LDS.32) and unpacked
-//     with PRMT straight into the float 2^23+v (bits 0x4B0000vv): differences
-//     of two such floats are exact.
-//   * idx = (int)(diff*wfact) and the test diff < diff_max collapse into
-//     FMUL.SAT by wfact/128 (power-of-two scaling is exact), FADD.RZ with 2^16
-//     (the mantissa then holds floor(128*t)), and a 129-entry table whose
-//     entries 127 and 128 are 0.  Valid while wfact < 0.99 (then diff >=
-//     diff_max implies idx >= 127); launch_plane() checks it.  No F2I.
+// Shared pieces of the fp32-exact kernels (nlmeans_v3.cuh, nlmeans_fast16_kernel): the same arithmetic results as
+// the kernel above, re-expressed for the SM's issue rates (CUDA C++ Programming Guide, arithmetic instruction
+// throughput, compute capability 9.0: FADD/FMUL/FFMA issue at 4 warp-instr/clk/SM, integer ALU ops at 2, F2I / I2F at
+// 0.5).
+//   * Samples are fetched as 32-bit words and unpacked with PRMT straight into the float 2^23+v (bits 0x4B0000vv):
+//     differences of two such floats are exact.
+//   * idx = (int)(diff*wfact) and the test diff < diff_max collapse into FMUL.SAT by wfact/128 (power-of-two scaling
+//     is exact), FADD.RZ with 2^16 (the mantissa then holds floor(128*t)), and a 129-entry table whose entries 127
+//     and 128 are 0.  Valid while wfact < 0.99 (then diff >= diff_max implies idx >= 127); the kernel selection checks
+//     it (table_trick_ok).  No F2I.
 // ---------------------------------------------------------------------------
 constexpr int kLutEntries = HBCU_NLMEANS_EXPSIZE + 1;
-
-template <int TH>
-struct FastLayout
-{
-    static constexpr int kRows      = TH + 2 * kHalo;
-    static constexpr int kTileBytes = kRows * kTilePW;
-    static constexpr int kAccBytes  = TH * kTileW * (int)sizeof(float);
-    static constexpr int kLutBytes  = kLutEntries * 32 * (int)sizeof(float);
-    static constexpr int kOffCur    = 0;
-    static constexpr int kOffCmp    = kOffCur + kTileBytes;
-    static constexpr int kOffWs     = kOffCmp + kTileBytes;
-    static constexpr int kOffPs     = kOffWs + kAccBytes;
-    static constexpr int kOffLut    = kOffPs + kAccBytes;
-    static constexpr int kOffBar    = kOffLut + kLutBytes;
-    static constexpr int kTotal     = kOffBar + 64;
-    static_assert(kTileBytes % 128 == 0, "TMA destination must stay 128-byte aligned");
-};
 
 // byte k (0..3) of word w as the float 2^23 + value
 __device__ __forceinline__ float byte_as_biased_float(uint32_t w, int k)
@@ -710,452 +686,11 @@ __device__ __forceinline__ float half_as_biased_float(uint32_t w, int k)
 
 #include "nlmeans_v3.cuh"
 
-template <int NH, int TH, int NW, bool ORIGIN>
-__device__ __forceinline__ void nlm_group_fast(const uint32_t *__restrict__ cur, const uint32_t *__restrict__ cmp,
-                                               float *__restrict__ acc_ws, float *__restrict__ acc_ps,
-                                               uint32_t lut_lane_addr, float wscale, double origin_tune,
-                                               int seg_y0, int lane, int dy, int dx0, int ng, int origin_g)
-{
-    constexpr int N   = 2 * NH + 1;
-    constexpr int RS  = TH / NW;
-    constexpr int NA  = 4 + 2 * NH;                 // source values per row
-    constexpr int NB  = NA + kGroup - 1;            // compare values per row
-    constexpr int PW  = kTilePW / 4;                // tile pitch in words
-    constexpr int OA  = (kHaloX - NH) & 3;          // byte offset of a[0] in its first word
-    constexpr int WA0 = (kHaloX - NH) >> 2;         // first word of the a window (relative to lane word)
-    constexpr int NWA = (OA + NA + 3) / 4;
-    constexpr int NWB = (NB + 3) / 4;               // aligned compare words
-    constexpr float kBias = 8388608.0f;             // 2^23
-
-    const int fb  = kHaloX - NH + dx0;              // first compare column relative to the lane's x
-    const int wb0 = fb >> 2;
-    const int ob  = (fb & 3) * 8;                   // funnel shift (bits) that aligns the compare window
-
-    float V[kGroup][4];
-    float hist[N][kGroup][4];
-#pragma unroll
-    for (int g = 0; g < kGroup; g++)
-#pragma unroll
-        for (int i = 0; i < 4; i++)
-        {
-            V[g][i] = 0.f;
-#pragma unroll
-            for (int k = 0; k < N; k++) hist[k][g][i] = 0.f;
-        }
-    // aligned compare words of the last NH rows: they hold the pixels cmp[y+dy][x+dx] of the
-    // output row that completes NH steps after its own compare row was loaded
-    uint32_t delay[NH][NWB];
-#pragma unroll
-    for (int r = 0; r < NH; r++)
-#pragma unroll
-        for (int j = 0; j < NWB; j++) delay[r][j] = 0;
-
-#pragma unroll 1
-    for (int base = -NH; base < RS + NH; base += N)
-    {
-#pragma unroll
-        for (int k = 0; k < N; k++)
-        {
-            const int yy = base + k;
-            if (yy < RS + NH)
-            {
-                const int ty = seg_y0 + yy + kHalo;
-                const uint32_t *aw = cur + ty * PW + lane + WA0;
-                const uint32_t *bw = cmp + (ty + dy) * PW + lane + wb0;
-                uint32_t wa[NWA], wraw[NWB + 1], wbv[NWB];
-#pragma unroll
-                for (int j = 0; j < NWA; j++) wa[j] = aw[j];
-#pragma unroll
-                for (int j = 0; j < NWB + 1; j++) wraw[j] = bw[j];
-#pragma unroll
-                for (int j = 0; j < NWB; j++) wbv[j] = __funnelshift_r(wraw[j], wraw[j + 1], ob);
-
-                float a[NA], b[NB];
-#pragma unroll
-                for (int j = 0; j < NA; j++) a[j] = byte_as_biased_float(wa[(OA + j) >> 2], (OA + j) & 3);
-#pragma unroll
-                for (int j = 0; j < NB; j++) b[j] = byte_as_biased_float(wbv[j >> 2], j & 3);
-
-#pragma unroll
-                for (int g = 0; g < kGroup; g++)
-                {
-                    if (g < ng && (!ORIGIN || g != origin_g))
-                    {
-                        float c[NA + 1];
-                        c[0] = 0.f;
-#pragma unroll
-                        for (int j = 0; j < NA; j++)
-                        {
-                            const float d = __fsub_rn(a[j], b[j + g]);        // exact
-                            c[j + 1] = __fmaf_rn(d, d, c[j]);                  // exact: integers < 2^24
-                        }
-#pragma unroll
-                        for (int i = 0; i < 4; i++)
-                        {
-                            const float hsum = __fsub_rn(c[i + N], c[i]);
-                            V[g][i] = __fadd_rn(V[g][i], __fsub_rn(hsum, hist[k][g][i]));
-                            hist[k][g][i] = hsum;
-                        }
-                    }
-                }
-                if (yy >= NH)
-                {
-                    const int oy = seg_y0 + yy - NH;
-                    float4 ws4 = *reinterpret_cast<float4 *>(acc_ws + oy * kTileW + lane * 4);
-                    float4 ps4 = *reinterpret_cast<float4 *>(acc_ps + oy * kTileW + lane * 4);
-                    float ws[4] = { ws4.x, ws4.y, ws4.z, ws4.w };
-                    float ps[4] = { ps4.x, ps4.y, ps4.z, ps4.w };
-                    // pixel values cmp[oy+dy][x+dx0+g+i] = element NH+g+i of the compare window loaded NH rows ago
-                    float pixv[kGroup + 3];
-#pragma unroll
-                    for (int j = 0; j < kGroup + 3; j++)
-                        pixv[j] = __fsub_rn(byte_as_biased_float(delay[0][(NH + j) >> 2], (NH + j) & 3), kBias);
-#pragma unroll
-                    for (int g = 0; g < kGroup; g++)
-                    {
-                        if (g < ng)
-                        {
-                            if (ORIGIN && g == origin_g)
-                            {
-                                const uint32_t cw = cur[(oy + kHalo) * PW + lane + kHaloX / 4];
-#pragma unroll
-                                for (int i = 0; i < 4; i++)
-                                    add_origin(ws[i], ps[i], origin_tune, (int)((cw >> (8 * i)) & 0xffu));
-                            }
-                            else
-                            {
-#pragma unroll
-                                for (int i = 0; i < 4; i++)
-                                {
-                                    float t, u, wgt;
-                                    asm("mul.rn.sat.f32 %0, %1, %2;" : "=f"(t) : "f"(V[g][i]), "f"(wscale));
-                                    asm("add.rz.f32 %0, %1, 0f47800000;" : "=f"(u) : "f"(t));   // 65536 + floor(128 t)
-                                    const uint32_t addr = (__float_as_uint(u) << 7) + lut_lane_addr;
-                                    asm("ld.shared.f32 %0, [%1];" : "=f"(wgt) : "r"(addr));
-                                    ws[i] = __fadd_rn(ws[i], wgt);
-                                    ps[i] = __fadd_rn(ps[i], __fmul_rn(wgt, pixv[g + i]));
-                                }
-                            }
-                        }
-                    }
-                    *reinterpret_cast<float4 *>(acc_ws + oy * kTileW + lane * 4) = make_float4(ws[0], ws[1], ws[2], ws[3]);
-                    *reinterpret_cast<float4 *>(acc_ps + oy * kTileW + lane * 4) = make_float4(ps[0], ps[1], ps[2], ps[3]);
-                }
-                // advance the delay line
-#pragma unroll
-                for (int r = 0; r + 1 < NH; r++)
-#pragma unroll
-                    for (int j = 0; j < NWB; j++) delay[r][j] = delay[r + 1][j];
-#pragma unroll
-                for (int j = 0; j < NWB; j++) delay[NH - 1][j] = wbv[j];
-            }
-        }
-    }
-}
-
-template <int NH, int TH, int NW, bool ORIGIN>
-__device__ __forceinline__ void nlm_group_dp4a(const uint32_t *__restrict__ cur, const uint32_t *__restrict__ cmp,
-                                               float *__restrict__ acc_ws, float *__restrict__ acc_ps,
-                                               uint32_t lut_lane_addr, float wscale, double origin_tune,
-                                               int seg_y0, int lane, int dy, int dx0, int ng, int origin_g)
-{
-    constexpr int N   = 2 * NH + 1;
-    constexpr int RS  = TH / NW;
-    constexpr int NA  = 4 + 2 * NH;                 // source values per row
-    constexpr int NB  = NA + kGroup - 1;            // compare values per row
-    constexpr int PW  = kTilePW / 4;                // tile pitch in words
-    constexpr int OA  = (kHaloX - NH) & 3;          // byte offset of a[0] in its first word
-    constexpr int WA0 = (kHaloX - NH) >> 2;         // first word of the a window (relative to lane word)
-    constexpr int NWA = (OA + NA + 3) / 4;
-    constexpr int NWB = (NB + 3) / 4;               // aligned compare words
-    constexpr float kBias = 8388608.0f;             // 2^23
-
-    const int fb  = kHaloX - NH + dx0;              // first compare column relative to the lane's x
-    const int wb0 = fb >> 2;
-    const int ob  = (fb & 3) * 8;                   // funnel shift (bits) that aligns the compare window
-
-    int V[kGroup][4];
-    int hist[N][kGroup][4];
-#pragma unroll
-    for (int g = 0; g < kGroup; g++)
-#pragma unroll
-        for (int i = 0; i < 4; i++)
-        {
-            V[g][i] = 0;
-#pragma unroll
-            for (int k = 0; k < N; k++) hist[k][g][i] = 0;
-        }
-    // aligned compare words of the last NH rows: they hold the pixels cmp[y+dy][x+dx] of the
-    // output row that completes NH steps after its own compare row was loaded
-    uint32_t delay[NH][NWB];
-#pragma unroll
-    for (int r = 0; r < NH; r++)
-#pragma unroll
-        for (int j = 0; j < NWB; j++) delay[r][j] = 0;
-
-#pragma unroll 1
-    for (int base = -NH; base < RS + NH; base += N)
-    {
-#pragma unroll
-        for (int k = 0; k < N; k++)
-        {
-            const int yy = base + k;
-            if (yy < RS + NH)
-            {
-                const int ty = seg_y0 + yy + kHalo;
-                const uint32_t *aw = cur + ty * PW + lane + WA0;
-                const uint32_t *bw = cmp + (ty + dy) * PW + lane + wb0;
-                uint32_t wa[NWA], wraw[NWB + 1], wbv[NWB];
-#pragma unroll
-                for (int j = 0; j < NWA; j++) wa[j] = aw[j];
-#pragma unroll
-                for (int j = 0; j < NWB + 1; j++) wraw[j] = bw[j];
-#pragma unroll
-                for (int j = 0; j < NWB; j++) wbv[j] = __funnelshift_r(wraw[j], wraw[j + 1], ob);
-
-                // Patch-row sums straight from the packed bytes: |a-b| for four pixels per VABSDIFF4, sums of
-                // squares over the 2NH+1 byte window per IDP4A (whole words) plus masked IDP4As for the partial
-                // words at both ends.  Integer-exact, no unpacking.
-                constexpr int NWD = (NA + 3) / 4;                    // words holding a[0..NA-1]
-                uint32_t aw4[NWD];
-#pragma unroll
-                for (int w = 0; w < NWD; w++)
-                    aw4[w] = OA ? __funnelshift_r(wa[w], (w + 1 < NWA) ? wa[w + 1] : 0u, 8 * OA) : wa[w];
-#pragma unroll
-                for (int g = 0; g < kGroup; g++)
-                {
-                    if (g < ng && (!ORIGIN || g != origin_g))
-                    {
-                        uint32_t D[NWD];
-#pragma unroll
-                        for (int w = 0; w < NWD; w++)
-                        {
-                            const uint32_t bg = g ? __funnelshift_r(wbv[w], (w + 1 < NWB) ? wbv[w + 1] : 0u, 8 * g) : wbv[w];
-                            D[w] = __vabsdiffu4(aw4[w], bg);
-                        }
-                        uint32_t T[NWD];
-#pragma unroll
-                        for (int w = 0; w < NWD; w++) T[w] = __dp4a(D[w], D[w], 0u);
-#pragma unroll
-                        for (int i = 0; i < 4; i++)
-                        {
-                            // window = bytes i .. i+N-1 of the D stream
-                            uint32_t acc = 0;
-                            bool started = false;
-#pragma unroll
-                            for (int w = 0; w < NWD; w++)
-                            {
-                                const int lo = max(i, 4 * w), hi = min(i + N - 1, 4 * w + 3);
-                                if (lo == 4 * w && hi == 4 * w + 3 && !started) { acc = T[w]; started = true; }
-                            }
-                            bool used_full = false;
-#pragma unroll
-                            for (int w = 0; w < NWD; w++)
-                            {
-                                const int lo = max(i, 4 * w), hi = min(i + N - 1, 4 * w + 3);
-                                if (lo > hi) continue;
-                                if (lo == 4 * w && hi == 4 * w + 3)
-                                {
-                                    if (started && !used_full) { used_full = true; continue; }   // already in acc
-                                    acc = __dp4a(D[w], D[w], acc);
-                                }
-                                else
-                                {
-                                    uint32_t m = 0;
-#pragma unroll
-                                    for (int bb = 0; bb < 4; bb++)
-                                        if (4 * w + bb >= lo && 4 * w + bb <= hi) m |= 0xFFu << (8 * bb);
-                                    acc = __dp4a(D[w] & m, D[w], acc);
-                                }
-                            }
-                            const int hsum = (int)acc;
-                            V[g][i] = V[g][i] + hsum - hist[k][g][i];
-                            hist[k][g][i] = hsum;
-                        }
-                    }
-                }
-                if (yy >= NH)
-                {
-                    const int oy = seg_y0 + yy - NH;
-                    float4 ws4 = *reinterpret_cast<float4 *>(acc_ws + oy * kTileW + lane * 4);
-                    float4 ps4 = *reinterpret_cast<float4 *>(acc_ps + oy * kTileW + lane * 4);
-                    float ws[4] = { ws4.x, ws4.y, ws4.z, ws4.w };
-                    float ps[4] = { ps4.x, ps4.y, ps4.z, ps4.w };
-                    // pixel values cmp[oy+dy][x+dx0+g+i] = element NH+g+i of the compare window loaded NH rows ago
-                    float pixv[kGroup + 3];
-#pragma unroll
-                    for (int j = 0; j < kGroup + 3; j++)
-                        pixv[j] = __fsub_rn(byte_as_biased_float(delay[0][(NH + j) >> 2], (NH + j) & 3), kBias);
-#pragma unroll
-                    for (int g = 0; g < kGroup; g++)
-                    {
-                        if (g < ng)
-                        {
-                            if (ORIGIN && g == origin_g)
-                            {
-                                const uint32_t cw = cur[(oy + kHalo) * PW + lane + kHaloX / 4];
-#pragma unroll
-                                for (int i = 0; i < 4; i++)
-                                    add_origin(ws[i], ps[i], origin_tune, (int)((cw >> (8 * i)) & 0xffu));
-                            }
-                            else
-                            {
-#pragma unroll
-                                for (int i = 0; i < 4; i++)
-                                {
-                                    float t, u, wgt;
-                                    asm("mul.rn.sat.f32 %0, %1, %2;" : "=f"(t) : "f"(__int2float_rn(V[g][i])), "f"(wscale));
-                                    asm("add.rz.f32 %0, %1, 0f47800000;" : "=f"(u) : "f"(t));   // 65536 + floor(128 t)
-                                    const uint32_t addr = (__float_as_uint(u) << 7) + lut_lane_addr;
-                                    asm("ld.shared.f32 %0, [%1];" : "=f"(wgt) : "r"(addr));
-                                    ws[i] = __fadd_rn(ws[i], wgt);
-                                    ps[i] = __fadd_rn(ps[i], __fmul_rn(wgt, pixv[g + i]));
-                                }
-                            }
-                        }
-                    }
-                    *reinterpret_cast<float4 *>(acc_ws + oy * kTileW + lane * 4) = make_float4(ws[0], ws[1], ws[2], ws[3]);
-                    *reinterpret_cast<float4 *>(acc_ps + oy * kTileW + lane * 4) = make_float4(ps[0], ps[1], ps[2], ps[3]);
-                }
-                // advance the delay line
-#pragma unroll
-                for (int r = 0; r + 1 < NH; r++)
-#pragma unroll
-                    for (int j = 0; j < NWB; j++) delay[r][j] = delay[r + 1][j];
-#pragma unroll
-                for (int j = 0; j < NWB; j++) delay[NH - 1][j] = wbv[j];
-            }
-        }
-    }
-}
-
-template <int NH, int TH, int NW, bool DP4A>
-__global__ void __launch_bounds__(NW * 32, 1) nlmeans_fast8_kernel(const __grid_constant__ FusedParams fp)
-{
-    constexpr int kThreads = NW * 32;
-    int pl = 0;
-    while (pl + 1 < fp.nplanes && (int)blockIdx.x >= fp.first_tile[pl + 1]) pl++;
-    const KernelParams &p = fp.k[pl];
-    const CUtensorMap *maps = fp.maps[pl];
-    const int tile = (int)blockIdx.x - fp.first_tile[pl];
-    using L = FastLayout<TH>;
-    extern __shared__ __align__(128) uint8_t smem[];
-    uint8_t *cur  = smem + L::kOffCur;
-    uint8_t *cmp  = smem + L::kOffCmp;
-    float *acc_ws = reinterpret_cast<float *>(smem + L::kOffWs);
-    float *acc_ps = reinterpret_cast<float *>(smem + L::kOffPs);
-    float *lut    = reinterpret_cast<float *>(smem + L::kOffLut);
-    uint64_t *bar = reinterpret_cast<uint64_t *>(smem + L::kOffBar);
-
-    const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
-    const int X0 = (tile % fp.tiles_x[pl]) * kTileW, Y0 = (tile / fp.tiles_x[pl]) * TH;
-    const int gx = X0 + kBorder - kHaloX, gy = Y0 + kBorder - kHalo;
-
-    if (tid == 0)
-    {
-        mbar_init(bar, 1);
-        asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
-    }
-    __syncthreads();
-    uint32_t phase = 0;
-    if (tid == 0)
-    {
-        mbar_expect_tx(bar, L::kTileBytes);
-        tma_load_2d(cur, &maps[0], gx, gy, bar);
-    }
-    for (int i = tid; i < kLutEntries * 32; i += kThreads)
-    {
-        const int e = i >> 5;
-        lut[i] = e < HBCU_NLMEANS_EXPSIZE ? p.exptable[e] : 0.f;
-    }
-    for (int i = tid; i < TH * kTileW; i += kThreads)
-    {
-        acc_ws[i] = 0.f;
-        acc_ps[i] = 0.f;
-    }
-    mbar_wait(bar, phase);
-    phase ^= 1;
-    __syncthreads();
-
-    const int seg_y0 = warp * (TH / NW);
-    const float wscale = p.wfact * 0.0078125f;                         // wfact / 128, exact
-    // shared address of this lane's copy of table entry 0, pre-biased by -(0x47800000 << 7)
-    const uint32_t lut_lane_addr = smem_u32(lut) + (uint32_t)lane * 4u - (0x47800000u << 7);
-    for (int f = 0; f < p.nf; f++)
-    {
-        const uint8_t *B = cur;
-        if (f > 0)
-        {
-            __syncthreads();
-            if (tid == 0)
-            {
-                fence_proxy_async();
-                mbar_expect_tx(bar, L::kTileBytes);
-                tma_load_2d(cmp, &maps[f], gx, gy, bar);
-            }
-            mbar_wait(bar, phase);
-            phase ^= 1;
-            B = cmp;
-        }
-        for (int dy = -p.r_half; dy <= p.r_half; dy++)
-        {
-            for (int dx0 = -p.r_half; dx0 <= p.r_half; dx0 += kGroup)
-            {
-                const int ng = min(kGroup, p.r_half - dx0 + 1);
-                const int origin_g = (f == 0 && dy == 0 && dx0 <= 0 && dx0 + ng > 0) ? -dx0 : -1;
-                // the origin variant (double-precision add of origin_tune) runs for one group per plane;
-                // keeping it out of the common instantiation keeps that loop body small
-                const uint32_t *cw = reinterpret_cast<const uint32_t *>(cur), *bw32 = reinterpret_cast<const uint32_t *>(B);
-                if (DP4A)
-                {
-                    if (origin_g >= 0)
-                        nlm_group_dp4a<NH, TH, NW, true>(cw, bw32, acc_ws, acc_ps, lut_lane_addr, wscale, p.origin_tune, seg_y0, lane, dy, dx0, ng, origin_g);
-                    else
-                        nlm_group_dp4a<NH, TH, NW, false>(cw, bw32, acc_ws, acc_ps, lut_lane_addr, wscale, p.origin_tune, seg_y0, lane, dy, dx0, ng, -1);
-                }
-                else
-                {
-                    if (origin_g >= 0)
-                        nlm_group_fast<NH, TH, NW, true>(cw, bw32, acc_ws, acc_ps, lut_lane_addr, wscale, p.origin_tune, seg_y0, lane, dy, dx0, ng, origin_g);
-                    else
-                        nlm_group_fast<NH, TH, NW, false>(cw, bw32, acc_ws, acc_ps, lut_lane_addr, wscale, p.origin_tune, seg_y0, lane, dy, dx0, ng, -1);
-                }
-            }
-        }
-    }
-
-    const int x = lane * 4;
-    uint8_t *dst = reinterpret_cast<uint8_t *>(p.dst);
-    for (int r = 0; r < TH / NW; r++)
-    {
-        const int oy = seg_y0 + r;
-        const int y = Y0 + oy;
-        if (y >= p.h) break;
-        const float4 ws4 = *reinterpret_cast<const float4 *>(acc_ws + oy * kTileW + x);
-        const float4 ps4 = *reinterpret_cast<const float4 *>(acc_ps + oy * kTileW + x);
-        const float ws[4] = { ws4.x, ws4.y, ws4.z, ws4.w };
-        const float ps[4] = { ps4.x, ps4.y, ps4.z, ps4.w };
-        uint8_t o[4];
-#pragma unroll
-        for (int i = 0; i < 4; i++)
-            o[i] = finish_pixel<uint8_t>(ws[i], ps[i], cur[(oy + kHalo) * kTilePW + x + kHaloX + i]);
-        uint8_t *drow = dst + (size_t)y * p.dpitch + X0 + x;
-        if (X0 + x + 3 < p.w)
-            *reinterpret_cast<uchar4 *>(drow) = make_uchar4(o[0], o[1], o[2], o[3]);
-        else
-        {
-#pragma unroll
-            for (int i = 0; i < 4; i++)
-                if (X0 + x + i < p.w) drow[i] = o[i];
-        }
-    }
-}
-
 // ---------------------------------------------------------------------------
 // Fast kernel for 9/10-bit planes (16-bit containers), patch <= 7.  Same tiling, same results.
 // With samples <= 1023 a squared difference is < 2^20, the prefix sum over the <= 10 values a lane touches
 // per row < 2^24 and one patch-row sum (7 * 1023^2) < 2^23, so the row sums are exact in fp32 (FSUB + FFMA per
-// pixel pair like the 8-bit fp32 variant).  The n x n sum (up to 5.1e7) is not, so the vertical running sum is an
+// pixel pair).  The n x n sum (up to 5.1e7) is not, so the vertical running sum is an
 // integer: hsum + 2^23 carries hsum in its mantissa bits and V += bits(new) - bits(old) is one IADD3 with no
 // unbiasing.  Samples travel as LDS.64 (4 samples; a warp reads 256 contiguous bytes, conflict free) and are
 // unpacked by PRMT into the float 2^23 + v.
@@ -1485,10 +1020,9 @@ struct hbcu_nlmeans_s
     std::vector<uint8_t *> out_mem;       // [oslot*3+plane]
     std::vector<int64_t>   ring_index;    // frame index held by each slot
     std::vector<CUtensorMap> maps;        // [slot*3+plane] TMA descriptors of the bordered planes
-    std::vector<CUtensorMap> maps3;       // same planes, box height of the v3 8-bit kernel's tile
+    std::vector<CUtensorMap> maps3;       // same planes, box height of the v3 kernels' tile (every v3 shape shares it)
     std::vector<CUtensorMap> maps3_pre;   // the prefiltered planes (pre_mem), same box
     std::vector<CUtensorMap> maps3f;      // same planes, box height of nlmeans_v3f_kernel's tile (v3_fused only)
-    int v3_nw, v3_rs;                     // v3 kernel shape (warps, rows per warp); v3_nw == 0: off
     bool v3_fused;                        // range 3 with nf <= 2 runs nlmeans_v3f_kernel (HBCU_NLMEANS_V3_FUSED=0: off)
     int v3f_rs;                           // its rows per warp (v3f_pick_rs), the box height of maps3f
     float *d_exptable;                    // 3 x 128
@@ -1523,191 +1057,11 @@ struct hbcu_nlmeans_s
 
 namespace {
 
-template <typename PIX, int NH, int TH>
-int launch_tiled(const TiledParams &kp, cudaStream_t st)
-{
-    using L = TileLayout<PIX, TH>;
-    // function attributes live in the device's context: one flag per device (a second GPU would otherwise launch with
-    // the default 48 KB limit -- 'invalid argument'; found by the first run of devices=0,1)
-    static bool configured_on[kMaxDevices] = {};
-    int dev_ = 0;
-    HBCU_CHECK(cudaGetDevice(&dev_));
-    bool &configured = configured_on[dev_ & (kMaxDevices - 1)];
-    if (!configured)
-    {
-        HBCU_CHECK(cudaFuncSetAttribute(nlmeans_tiled_kernel<PIX, NH, TH>,
-                                        cudaFuncAttributeMaxDynamicSharedMemorySize, L::kTotal));
-        configured = true;
-    }
-    dim3 grid((kp.k.w + kTileW - 1) / kTileW, (kp.k.h + TH - 1) / TH);
-    nlmeans_tiled_kernel<PIX, NH, TH><<<grid, kThreads, L::kTotal, st>>>(kp);
-    hbcu::count_launch();
-    return 0;
-}
-
-template <int NH, int TH, int NW, bool DP4A>
-int launch_fast8(FusedParams &fp, cudaStream_t st)
-{
-    using L = FastLayout<TH>;
-    // function attributes live in the device's context: one flag per device (a second GPU would otherwise launch with
-    // the default 48 KB limit -- 'invalid argument'; found by the first run of devices=0,1)
-    static bool configured_on[kMaxDevices] = {};
-    int dev_ = 0;
-    HBCU_CHECK(cudaGetDevice(&dev_));
-    bool &configured = configured_on[dev_ & (kMaxDevices - 1)];
-    if (!configured)
-    {
-        HBCU_CHECK(cudaFuncSetAttribute(nlmeans_fast8_kernel<NH, TH, NW, DP4A>, cudaFuncAttributeMaxDynamicSharedMemorySize, L::kTotal));
-        configured = true;
-    }
-    int total = 0;
-    for (int i = 0; i < fp.nplanes; i++)
-    {
-        fp.first_tile[i] = total;
-        fp.tiles_x[i] = (fp.k[i].w + kTileW - 1) / kTileW;
-        total += fp.tiles_x[i] * ((fp.k[i].h + TH - 1) / TH);
-    }
-    fp.first_tile[fp.nplanes] = total;
-    nlmeans_fast8_kernel<NH, TH, NW, DP4A><<<total, NW * 32, L::kTotal, st>>>(fp);
-    hbcu::count_launch();
-    return 0;
-}
-
-template <int NH, int TH, int NW>
-int launch_fast16(FusedParams &fp, cudaStream_t st)
-{
-    using L = Fast16Layout<TH>;
-    // function attributes live in the device's context: one flag per device (a second GPU would otherwise launch with
-    // the default 48 KB limit -- 'invalid argument'; found by the first run of devices=0,1)
-    static bool configured_on[kMaxDevices] = {};
-    int dev_ = 0;
-    HBCU_CHECK(cudaGetDevice(&dev_));
-    bool &configured = configured_on[dev_ & (kMaxDevices - 1)];
-    if (!configured)
-    {
-        HBCU_CHECK(cudaFuncSetAttribute(nlmeans_fast16_kernel<NH, TH, NW>, cudaFuncAttributeMaxDynamicSharedMemorySize, L::kTotal));
-        configured = true;
-    }
-    int total = 0;
-    for (int i = 0; i < fp.nplanes; i++)
-    {
-        fp.first_tile[i] = total;
-        fp.tiles_x[i] = (fp.k[i].w + kTileW - 1) / kTileW;
-        total += fp.tiles_x[i] * ((fp.k[i].h + TH - 1) / TH);
-    }
-    fp.first_tile[fp.nplanes] = total;
-    nlmeans_fast16_kernel<NH, TH, NW><<<total, NW * 32, L::kTotal, st>>>(fp);
-    hbcu::count_launch();
-    return 0;
-}
-
 // 16-bit tiles are 128 x 96 for every kernel (they share the tensor maps): 8 warps x 12 rows
 constexpr int kTH16 = 96;
 
-int launch_fast16_nh(FusedParams &kp, cudaStream_t st)
-{
-    switch (kp.k[0].n_half)
-    {
-        case 1: return launch_fast16<1, kTH16, 8>(kp, st);
-        case 2: return launch_fast16<2, kTH16, 8>(kp, st);
-        case 3: return launch_fast16<3, kTH16, 8>(kp, st);
-        default: return 1;
-    }
-}
-
-// 8-bit tiles are 128 x 144: 12 warps x 12 rows for patch <= 7 (measured 7 % faster than 8 warps x 16 rows:
-// more warps hide the dependent-issue latency better than the extra warm-up rows cost), 8 warps x 18 rows
-// for patch 9 whose register footprint does not allow 384 threads.
+// 8-bit tiles of the integer tiled kernel are 128 x 144 (8 warps x 18 rows); an 8-bit handle's `maps` have that box
 constexpr int kTH8 = 144;
-
-int g_ssd_variant = 1;     // 1: packed-byte VABSDIFF4 + IDP4A patch-row sums (measured 7 % faster), 0: fp32 prefix sums (FFMA);
-                           // HBCU_NLMEANS_SSD selects (test/tuning hook: both are exact, tests run both)
-
-template <int NH, int NW, int RS, int NBUF, bool SYM = false>
-int launch_v3(FusedParams &fp, cudaStream_t st)
-{
-    using L = V3Layout<NW, RS, NBUF>;
-    // function attributes live in the device's context: one flag per device (a second GPU would otherwise launch with
-    // the default 48 KB limit -- 'invalid argument'; found by the first run of devices=0,1)
-    static bool configured_on[kMaxDevices] = {};
-    int dev_ = 0;
-    HBCU_CHECK(cudaGetDevice(&dev_));
-    bool &configured = configured_on[dev_ & (kMaxDevices - 1)];
-    if (!configured)
-    {
-        HBCU_CHECK(cudaFuncSetAttribute(nlmeans_v3_kernel<NH, NW, RS, NBUF, false, SYM>, cudaFuncAttributeMaxDynamicSharedMemorySize, L::kTotal));
-        configured = true;
-    }
-    int total = 0;
-    for (int i = 0; i < fp.nplanes; i++)
-    {
-        fp.first_tile[i] = total;
-        fp.tiles_x[i] = (fp.k[i].w + kTileW - 1) / kTileW;
-        total += fp.tiles_x[i] * ((fp.k[i].h + L::kTH - 1) / L::kTH);
-    }
-    fp.first_tile[fp.nplanes] = total;
-    nlmeans_v3_kernel<NH, NW, RS, NBUF, false, SYM><<<total, NW * 32, L::kTotal, st>>>(fp);
-    hbcu::count_launch();
-    return 0;
-}
-
-template <int NH, int NW, int RS, int NBUF>
-int launch_v3w(FusedParams &fp, cudaStream_t st)
-{
-    using L = V3Layout<NW, RS, NBUF, 2>;
-    // function attributes live in the device's context: one flag per device (a second GPU would otherwise launch with
-    // the default 48 KB limit -- 'invalid argument'; found by the first run of devices=0,1)
-    static bool configured_on[kMaxDevices] = {};
-    int dev_ = 0;
-    HBCU_CHECK(cudaGetDevice(&dev_));
-    bool &configured = configured_on[dev_ & (kMaxDevices - 1)];
-    if (!configured)
-    {
-        HBCU_CHECK(cudaFuncSetAttribute(nlmeans_v3w_kernel<NH, NW, RS, NBUF>, cudaFuncAttributeMaxDynamicSharedMemorySize, L::kTotal));
-        configured = true;
-    }
-    int total = 0;
-    for (int i = 0; i < fp.nplanes; i++)
-    {
-        fp.first_tile[i] = total;
-        fp.tiles_x[i] = (fp.k[i].w + kTileW - 1) / kTileW;
-        total += fp.tiles_x[i] * ((fp.k[i].h + L::kTH - 1) / L::kTH);
-    }
-    fp.first_tile[fp.nplanes] = total;
-    nlmeans_v3w_kernel<NH, NW, RS, NBUF><<<total, NW * 32, L::kTotal, st>>>(fp);
-    hbcu::count_launch();
-    return 0;
-}
-
-// prefilter variant (patch distances from the pre-denoised planes): one plane per launch, 12 x 10, one compare buffer pair
-template <int NH>
-int launch_v3_pre(FusedParams &fp, cudaStream_t st)
-{
-    constexpr int NW = 12, RS = 10;
-    using L = V3Layout<NW, RS, 1, 1, true>;
-    // function attributes live in the device's context: one flag per device (a second GPU would otherwise launch with
-    // the default 48 KB limit -- 'invalid argument'; found by the first run of devices=0,1)
-    static bool configured_on[kMaxDevices] = {};
-    int dev_ = 0;
-    HBCU_CHECK(cudaGetDevice(&dev_));
-    bool &configured = configured_on[dev_ & (kMaxDevices - 1)];
-    if (!configured)
-    {
-        HBCU_CHECK(cudaFuncSetAttribute(nlmeans_v3_kernel<NH, NW, RS, 1, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, L::kTotal));
-        configured = true;
-    }
-    int total = 0;
-    for (int i = 0; i < fp.nplanes; i++)
-    {
-        fp.first_tile[i] = total;
-        fp.tiles_x[i] = (fp.k[i].w + kTileW - 1) / kTileW;
-        total += fp.tiles_x[i] * ((fp.k[i].h + L::kTH - 1) / L::kTH);
-    }
-    fp.first_tile[fp.nplanes] = total;
-    nlmeans_v3_kernel<NH, NW, RS, 1, true><<<total, NW * 32, L::kTotal, st>>>(fp);
-    hbcu::count_launch();
-    return 0;
-}
 
 // v3 shapes built into the library: {warps, rows per warp}.  Every variant has a 120-row tile (see V3Layout: the
 // shared-memory accumulators and tiles of the 16-bit and prefilter variants fill 221 KB of the 227 KB).  Patch 9
@@ -1722,6 +1076,7 @@ constexpr V3Shape kV3Fused = { 12, 20 };
 constexpr V3Shape kV3FusedTall = { 12, 30 };
 constexpr V3Shape kV3FusedTaller = { 12, 45 };
 constexpr int kV3FusedWarmRows = 7;      // 2 NH + 1 at patch 7: the warm-up rows the shape rule charges each strip
+static_assert(kV3Fused.nw == kV3FusedTall.nw && kV3Fused.nw == kV3FusedTaller.nw, "one warp count");
 
 // CTAs of one frame (all three planes) in nlmeans_v3f_kernel at strips of rs rows
 int v3f_tiles(const PlaneGeom *g, int rs)
@@ -1745,273 +1100,291 @@ int v3f_pick_rs(const PlaneGeom *g, int sms)
     return v3f_tiles(g, kV3FusedTall.rs) >= sms ? kV3FusedTall.rs : kV3Fused.rs;
 }
 
-template <int NH, int RS>
-int launch_v3f(FusedParams &fp, cudaStream_t st)
-{
-    constexpr int NW = kV3Fused.nw;
-    using L = V3FusedLayout<NW, RS>;
-    // function attributes live in the device's context: one flag per device
-    static bool configured_on[kMaxDevices] = {};
-    int dev_ = 0;
-    HBCU_CHECK(cudaGetDevice(&dev_));
-    bool &configured = configured_on[dev_ & (kMaxDevices - 1)];
-    if (!configured)
-    {
-        HBCU_CHECK(cudaFuncSetAttribute(nlmeans_v3f_kernel<NH, NW, RS>, cudaFuncAttributeMaxDynamicSharedMemorySize, L::kTotal));
-        configured = true;
-    }
-    int total = 0;
-    for (int i = 0; i < fp.nplanes; i++)
-    {
-        fp.first_tile[i] = total;
-        fp.tiles_x[i] = (fp.k[i].w + kTileW - 1) / kTileW;
-        total += fp.tiles_x[i] * ((fp.k[i].h + L::kTH - 1) / L::kTH);
-    }
-    fp.first_tile[fp.nplanes] = total;
-    nlmeans_v3f_kernel<NH, NW, RS><<<total, NW * 32, L::kTotal, st>>>(fp);
-    hbcu::count_launch();
-    return 0;
-}
-
-// nlmeans_v3f_kernel takes a launch whose planes all have range 3 and one or two frames (patch 3 .. 7; the caller has
-// checked that the 8-bit v3 kernel may run them).  More frames keep the accumulating kernel: each further frame would
-// add nine running sums to registers that are full.
-bool v3f_ok(const hbcu_nlmeans_s *h, const KernelParams *kps, const bool *active, int n)
-{
-    if (!h->v3_fused) return false;
-    bool any = false;
-    for (int pl = 0; pl < n; pl++)
-    {
-        if (active != nullptr && !active[pl]) continue;
-        const KernelParams &k = kps[pl];
-        if (k.r_half != 1 || k.nf > 2 || k.n_half < 1 || k.n_half > 3 || k.use_pre) return false;
-        any = true;
-    }
-    return any;
-}
-
-template <int RS>
-int launch_v3f_rs(FusedParams &fp, cudaStream_t st)
-{
-    const int nh = fp.k[0].n_half;
-    if (nh == 1) return launch_v3f<1, RS>(fp, st);
-    if (nh == 2) return launch_v3f<2, RS>(fp, st);
-    if (nh == 3) return launch_v3f<3, RS>(fp, st);
-    return 1;
-}
-
-int launch_v3f_nh(int rs, FusedParams &fp, cudaStream_t st)
-{
-    static_assert(kV3Fused.nw == kV3FusedTall.nw && kV3Fused.nw == kV3FusedTaller.nw, "one warp count");
-    if (rs == kV3FusedTaller.rs) return launch_v3f_rs<kV3FusedTaller.rs>(fp, st);
-    if (rs == kV3FusedTall.rs) return launch_v3f_rs<kV3FusedTall.rs>(fp, st);
-    return launch_v3f_rs<kV3Fused.rs>(fp, st);
-}
-
 // rows of one TMA box of the v3 tile: V3Layout::kBoxRows restated for a run-time shape (the kernel's expect-tx byte
 // count and the tensor map must agree)
-int v3_box_rows(int nw, int rs)
+constexpr int v3_box_rows(int nw, int rs)
 {
     const int rows = nw * rs + 2 * kHalo, loads = (rows + 255) / 256;
     return ((rows + loads - 1) / loads + 3) / 4 * 4;
 }
 
-bool v3_shape_ok(int nw, int rs, int n_half)
-{
-    if (n_half == 4) return nw == 8 && rs == 15;
-    return nw == kV3Default.nw && rs == kV3Default.rs;
-}
-
-// the shape a plane with patch half-width n_half runs in, given the handle's shape (whose TMA box its tensor maps
-// were encoded for): patch 9 takes the 8-warp shape with the same tile height as 12 x 10
-bool v3_pick(const hbcu_nlmeans_s *h, int n_half, V3Shape *out)
-{
-    if (h->v3_nw <= 0) return false;
-    V3Shape s = { h->v3_nw, h->v3_rs };
-    if (n_half == 4)
-    {
-        s = V3Shape{ 8, 15 };
-        if (v3_box_rows(s.nw, s.rs) != v3_box_rows(h->v3_nw, h->v3_rs) || s.nw * s.rs != h->v3_nw * h->v3_rs) return false;
-    }
-    if (!v3_shape_ok(s.nw, s.rs, n_half)) return false;
-    *out = s;
-    return true;
-}
-
-int launch_v3_nh(int nw, int rs, FusedParams &fp, cudaStream_t st)
-{
-    const int nh = fp.k[0].n_half;
-    // every displacement row of this range must decompose into group shapes the kernels were built with
-    for (int pl = 0; pl < fp.nplanes; pl++)
-        for (int dx0 = -fp.k[pl].r_half; dx0 <= fp.k[pl].r_half; dx0 += kGroup)
-        {
-            const int ng = std::min(kGroup, fp.k[pl].r_half - dx0 + 1);
-            if (!v3_group_known(ng, (12 + dx0) & 3, kOrgNone)) return 1;
-            if (dx0 <= 0 && dx0 + ng > 0 && !v3_group_known(ng, (12 + dx0) & 3, -dx0)) return 1;
-        }
-    // range 3 in every plane: frame 0 runs as one symmetric march (V3Sym, nlmeans_v3.cuh)
-    bool sym = true;
-    for (int pl = 0; pl < fp.nplanes; pl++) sym = sym && fp.k[pl].r_half == 1;
-    if (sym && nw == 12 && rs == 10)
-    {
-        if (nh == 1) return launch_v3<1, 12, 10, 2, true>(fp, st);
-        if (nh == 2) return launch_v3<2, 12, 10, 2, true>(fp, st);
-        if (nh == 3) return launch_v3<3, 12, 10, 2, true>(fp, st);
-    }
-#define V3CASE(NH_, NW_, RS_, NB_) if (nh == NH_ && nw == NW_ && rs == RS_) return launch_v3<NH_, NW_, RS_, NB_>(fp, st)
-    V3CASE(1, 12, 10, 2); V3CASE(2, 12, 10, 2); V3CASE(3, 12, 10, 2);
-    V3CASE(4, 8, 15, 2);
-#undef V3CASE
-    return 1;
-}
-
 // 16-bit planes: one shape (12 warps x 10 rows, one compare buffer: two 42.5 KB tiles)
 constexpr V3Shape kV3wShape = { 12, 10 };
 
-int launch_v3w_nh(FusedParams &fp, cudaStream_t st)
-{
-    for (int pl = 0; pl < fp.nplanes; pl++)
-        for (int dx0 = -fp.k[pl].r_half; dx0 <= fp.k[pl].r_half; dx0 += kGroup)
-        {
-            const int ng = std::min(kGroup, fp.k[pl].r_half - dx0 + 1);
-            if (!v3_group_known(ng, (12 + dx0) & 3, kOrgNone)) return 1;
-            if (dx0 <= 0 && dx0 + ng > 0 && !v3_group_known(ng, (12 + dx0) & 3, -dx0)) return 1;
-        }
-    switch (fp.k[0].n_half)
-    {
-        case 1: return launch_v3w<1, kV3wShape.nw, kV3wShape.rs, 1>(fp, st);
-        case 2: return launch_v3w<2, kV3wShape.nw, kV3wShape.rs, 1>(fp, st);
-        case 3: return launch_v3w<3, kV3wShape.nw, kV3wShape.rs, 1>(fp, st);
-        default: return 1;
-    }
-}
+// the 8-bit v3 shape of a plane with patch half-width n_half: patch 9 takes the 8-warp shape
+constexpr V3Shape v3_shape(int n_half) { return n_half == 4 ? V3Shape{ 8, 15 } : kV3Default; }
 
-int launch_fast8_nh(FusedParams &kp, cudaStream_t st)
+// every v3 kernel reads the tensor maps maps3, encoded for kV3Default: a shape must keep its tile height and box rows
+constexpr bool v3_shares_maps3(V3Shape s)
 {
-    if (g_ssd_variant == 1)
-    {
-        switch (kp.k[0].n_half)
-        {
-            case 1: return launch_fast8<1, kTH8, 12, true>(kp, st);
-            case 2: return launch_fast8<2, kTH8, 12, true>(kp, st);
-            case 3: return launch_fast8<3, kTH8, 12, true>(kp, st);
-            case 4: return launch_fast8<4, kTH8, 8, true>(kp, st);
-            default: return 1;
-        }
-    }
-    switch (kp.k[0].n_half)
-    {
-        case 1: return launch_fast8<1, kTH8, 12, false>(kp, st);
-        case 2: return launch_fast8<2, kTH8, 12, false>(kp, st);
-        case 3: return launch_fast8<3, kTH8, 12, false>(kp, st);
-        case 4: return launch_fast8<4, kTH8, 8, false>(kp, st);
-        default: return 1;
-    }
+    return s.nw * s.rs == kV3Default.nw * kV3Default.rs && v3_box_rows(s.nw, s.rs) == v3_box_rows(kV3Default.nw, kV3Default.rs);
 }
+static_assert(v3_shares_maps3(v3_shape(4)) && v3_shares_maps3(kV3wShape), "the v3 shapes share maps3");
 
-template <typename PIX, int TH>
-int launch_tiled_nh(const TiledParams &kp, cudaStream_t st)
+// the active planes of one frame as run_filter set them up, and the ring slot of each frame a plane reads
+struct FramePlanes
 {
-    switch (kp.k.n_half)
+    KernelParams k[3];
+    int slots[3][kMaxFrames];
+    bool active[3];
+};
+
+struct Launch;
+using Runner = int (*)(hbcu_nlmeans_s *h, const FramePlanes &fr, const Launch &l);
+
+// one kernel launch of a frame: the launcher of one kernel instantiation and the planes it covers
+struct Launch
+{
+    Runner run;
+    int nplanes;
+    int plane[3];
+    bool if_flag;     // the integer tiled kernel behind a fused 16-bit launch: runs only if the border kernel raised the
+                      // range flag, and is not counted in kernel_launches
+};
+
+// Function attributes live in the device's context: one flag per kernel and device (a second GPU would otherwise launch
+// with the default 48 KB limit -- 'invalid argument'; found by the first run of devices=0,1)
+template <auto K>
+int opt_in_smem(int bytes)
+{
+    static bool configured_on[kMaxDevices] = {};
+    int dev = 0;
+    HBCU_CHECK(cudaGetDevice(&dev));
+    bool &configured = configured_on[dev & (kMaxDevices - 1)];
+    if (!configured)
     {
-        case 1: return launch_tiled<PIX, 1, TH>(kp, st);
-        case 2: return launch_tiled<PIX, 2, TH>(kp, st);
-        case 3: return launch_tiled<PIX, 3, TH>(kp, st);
-        case 4: return launch_tiled<PIX, 4, TH>(kp, st);
-        default: return 1;
+        HBCU_CHECK(cudaFuncSetAttribute(K, cudaFuncAttributeMaxDynamicSharedMemorySize, bytes));
+        configured = true;
     }
-}
-
-bool tiled_supported(const KernelParams &kp)
-{
-    return !kp.use_pre && kp.n_half >= 1 && kp.n_half <= 4 && kp.n_half + kp.r_half <= kHalo && kp.nf <= kMaxTiledFrames;
-}
-
-bool fast8_ok(const hbcu_nlmeans_s *h, const KernelParams &kp)
-{
-    // fp32-exact fast kernel: 8-bit planes, halo fits, the saturating table trick is valid (wfact < 0.99)
-    return h->bps == 1 && h->impl != 1 && h->impl != 3 && tiled_supported(kp) && kp.wfact < 0.99f && kp.wfact > 1e-5f;
-}
-
-bool fast16_ok(const hbcu_nlmeans_s *h, const KernelParams &kp)
-{
-    // fp32-exact fast kernel for 9/10-bit planes: patch <= 7, same table trick
-    return h->bps == 2 && h->cfg.depth <= 10 && h->impl != 1 && h->impl != 3 && tiled_supported(kp) && kp.n_half <= 3 &&
-           kp.wfact < 0.99f && kp.wfact > 1e-5f;
-}
-
-int launch_plane(hbcu_nlmeans_s *h, const KernelParams &kp, const int *slots, int plane, const unsigned *only_if_flag = nullptr)
-{
-    // prefilter modes on 8-bit planes: the v3 kernel's prefilter variant (VERDICT r1 missing 5: these settings used to fall
-    // to the one-thread-per-pixel generic kernel); same validity conditions as the plain fast kernel
-    if (kp.use_pre && only_if_flag == nullptr && h->bps == 1 && h->impl == 0 && h->v3_nw == kV3Default.nw && h->v3_rs == kV3Default.rs &&
-        kp.n_half >= 1 && kp.n_half <= 3 && kp.n_half + kp.r_half <= kHalo && kp.nf <= kMaxTiledFrames && kp.wfact < 0.99f && kp.wfact > 1e-5f)
-    {
-        bool known = true;
-        for (int dx0 = -kp.r_half; dx0 <= kp.r_half; dx0 += kGroup)
-        {
-            const int ng = std::min(kGroup, kp.r_half - dx0 + 1);
-            known = known && v3_group_known(ng, (12 + dx0) & 3, kOrgNone) && (!(dx0 <= 0 && dx0 + ng > 0) || v3_group_known(ng, (12 + dx0) & 3, -dx0));
-        }
-        if (known)
-        {
-            FusedParams fp;
-            fp.nplanes = 1;
-            fp.range_flag = nullptr;
-            fp.k[0] = kp;
-            for (int f = 0; f < kp.nf; f++)
-            {
-                fp.maps[0][f] = h->maps3[slots[f] * 3 + plane];
-                fp.maps_pre[0][f] = h->maps3_pre[slots[f] * 3 + plane];
-            }
-            const int rc = kp.n_half == 1 ? launch_v3_pre<1>(fp, h->s_compute) : kp.n_half == 2 ? launch_v3_pre<2>(fp, h->s_compute) : launch_v3_pre<3>(fp, h->s_compute);
-            if (rc != 0) return rc;
-            HBCU_CHECK(cudaGetLastError());
-            return 0;
-        }
-    }
-    const bool want_tiled = h->impl != 1 && tiled_supported(kp);
-    if (h->impl == 2 && !want_tiled)
-    {
-        set_error("nlmeans: tiled kernel does not support n=%d r=%d", 2 * kp.n_half + 1, 2 * kp.r_half + 1);
-        return -1;
-    }
-    if (want_tiled)
-    {
-        TiledParams tp;
-        tp.k = kp;
-        tp.only_if_flag = only_if_flag;
-        for (int f = 0; f < kp.nf; f++) tp.maps[f] = h->maps[slots[f] * 3 + plane];
-        // impl 0/2: fp32-exact fast kernel for 8-bit planes when the table trick is valid; impl 3: integer tiled kernel
-        const bool fast_ok = fast8_ok(h, kp);
-        int rc;
-        if (fast_ok && h->impl != 3)
-        {
-            FusedParams fp;
-            fp.nplanes = 1;
-            fp.range_flag = nullptr;
-            fp.k[0] = kp;
-            V3Shape vs;
-            const bool v3 = v3_pick(h, kp.n_half, &vs);
-            const bool v3f = v3 && v3f_ok(h, &kp, nullptr, 1);
-            for (int f = 0; f < kp.nf; f++) fp.maps[0][f] = v3f ? h->maps3f[slots[f] * 3 + plane] : v3 ? h->maps3[slots[f] * 3 + plane] : tp.maps[f];
-            rc = v3f ? launch_v3f_nh(h->v3f_rs, fp, h->s_compute) : v3 ? launch_v3_nh(vs.nw, vs.rs, fp, h->s_compute) : launch_fast8_nh(fp, h->s_compute);
-        }
-        else
-            rc = h->bps == 1 ? launch_tiled_nh<uint8_t, kTH8>(tp, h->s_compute) : launch_tiled_nh<uint16_t, kTH16>(tp, h->s_compute);
-        if (rc < 0) return rc;
-        if (rc == 0)
-        {
-            HBCU_CHECK(cudaGetLastError());
-            return 0;
-        }
-    }
-    dim3 blk(32, 8), grid((kp.w + 31) / 32, (kp.h + 7) / 8);
-    if (h->bps == 1) nlmeans_generic_kernel<uint8_t><<<grid, blk, 0, h->s_compute>>>(kp);
-    else             nlmeans_generic_kernel<uint16_t><<<grid, blk, 0, h->s_compute>>>(kp);
-    hbcu::count_launch();
-    HBCU_CHECK(cudaGetLastError());
     return 0;
+}
+
+// a fused-grid kernel: the tiles (tile_rows high) of every plane of fp in one linear grid, plane after plane
+template <auto K>
+int launch_tiles(FusedParams &fp, int tile_rows, int smem, int threads, cudaStream_t st)
+{
+    if (opt_in_smem<K>(smem) != 0) return -1;
+    int total = 0;
+    for (int i = 0; i < fp.nplanes; i++)
+    {
+        fp.first_tile[i] = total;
+        fp.tiles_x[i] = (fp.k[i].w + kTileW - 1) / kTileW;
+        total += fp.tiles_x[i] * ((fp.k[i].h + tile_rows - 1) / tile_rows);
+    }
+    fp.first_tile[fp.nplanes] = total;
+    K<<<total, threads, smem, st>>>(fp);
+    hbcu::count_launch();
+    return 0;
+}
+
+// the FusedParams of a launch: its planes and the tensor maps of their frames from `maps` (and `maps_pre`)
+FusedParams fused_params(const hbcu_nlmeans_s *h, const FramePlanes &fr, const Launch &l, const std::vector<CUtensorMap> &maps,
+                         const std::vector<CUtensorMap> *maps_pre = nullptr)
+{
+    FusedParams fp;
+    fp.nplanes = l.nplanes;
+    fp.range_flag = h->d_range_flag;
+    for (int i = 0; i < l.nplanes; i++)
+    {
+        const int pl = l.plane[i];
+        fp.k[i] = fr.k[pl];
+        for (int f = 0; f < fr.k[pl].nf; f++)
+        {
+            fp.maps[i][f] = maps[fr.slots[pl][f] * 3 + pl];
+            if (maps_pre != nullptr) fp.maps_pre[i][f] = (*maps_pre)[fr.slots[pl][f] * 3 + pl];
+        }
+    }
+    return fp;
+}
+
+template <int NH, bool SYM>
+int launch_v3(hbcu_nlmeans_s *h, const FramePlanes &fr, const Launch &l)
+{
+    constexpr V3Shape s = v3_shape(NH);
+    using L = V3Layout<s.nw, s.rs, 2>;
+    FusedParams fp = fused_params(h, fr, l, h->maps3);
+    return launch_tiles<nlmeans_v3_kernel<NH, s.nw, s.rs, 2, false, SYM>>(fp, L::kTH, L::kTotal, s.nw * 32, h->s_compute);
+}
+
+// prefilter variant (patch distances from the pre-denoised planes): one plane per launch, one compare buffer pair
+template <int NH>
+int launch_v3_pre(hbcu_nlmeans_s *h, const FramePlanes &fr, const Launch &l)
+{
+    using L = V3Layout<kV3Default.nw, kV3Default.rs, 1, 1, true>;
+    FusedParams fp = fused_params(h, fr, l, h->maps3, &h->maps3_pre);
+    return launch_tiles<nlmeans_v3_kernel<NH, kV3Default.nw, kV3Default.rs, 1, true>>(fp, L::kTH, L::kTotal, kV3Default.nw * 32, h->s_compute);
+}
+
+template <int NH, int RS>
+int launch_v3f(hbcu_nlmeans_s *h, const FramePlanes &fr, const Launch &l)
+{
+    using L = V3FusedLayout<kV3Fused.nw, RS>;
+    FusedParams fp = fused_params(h, fr, l, h->maps3f);
+    return launch_tiles<nlmeans_v3f_kernel<NH, kV3Fused.nw, RS>>(fp, L::kTH, L::kTotal, kV3Fused.nw * 32, h->s_compute);
+}
+
+template <int NH>
+int launch_v3w(hbcu_nlmeans_s *h, const FramePlanes &fr, const Launch &l)
+{
+    using L = V3Layout<kV3wShape.nw, kV3wShape.rs, 1, 2>;
+    FusedParams fp = fused_params(h, fr, l, h->maps3);
+    return launch_tiles<nlmeans_v3w_kernel<NH, kV3wShape.nw, kV3wShape.rs, 1>>(fp, L::kTH, L::kTotal, kV3wShape.nw * 32, h->s_compute);
+}
+
+template <int NH>
+int launch_fast16(hbcu_nlmeans_s *h, const FramePlanes &fr, const Launch &l)
+{
+    FusedParams fp = fused_params(h, fr, l, h->maps);
+    return launch_tiles<nlmeans_fast16_kernel<NH, kTH16, 8>>(fp, kTH16, Fast16Layout<kTH16>::kTotal, 8 * 32, h->s_compute);
+}
+
+template <typename PIX, int NH>
+int launch_tiled(hbcu_nlmeans_s *h, const FramePlanes &fr, const Launch &l)
+{
+    constexpr int TH = sizeof(PIX) == 1 ? kTH8 : kTH16;
+    using L = TileLayout<PIX, TH>;
+    const int pl = l.plane[0];
+    TiledParams tp;
+    tp.k = fr.k[pl];
+    tp.only_if_flag = l.if_flag ? h->d_range_flag : nullptr;
+    for (int f = 0; f < tp.k.nf; f++) tp.maps[f] = h->maps[fr.slots[pl][f] * 3 + pl];
+    if (opt_in_smem<nlmeans_tiled_kernel<PIX, NH, TH>>(L::kTotal) != 0) return -1;
+    dim3 grid((tp.k.w + kTileW - 1) / kTileW, (tp.k.h + TH - 1) / TH);
+    nlmeans_tiled_kernel<PIX, NH, TH><<<grid, kThreads, L::kTotal, h->s_compute>>>(tp);
+    hbcu::count_launch();
+    return 0;
+}
+
+template <typename PIX>
+int launch_generic(hbcu_nlmeans_s *h, const FramePlanes &fr, const Launch &l)
+{
+    const KernelParams &k = fr.k[l.plane[0]];
+    dim3 blk(32, 8), grid((k.w + 31) / 32, (k.h + 7) / 8);
+    nlmeans_generic_kernel<PIX><<<grid, blk, 0, h->s_compute>>>(k);
+    hbcu::count_launch();
+    return 0;
+}
+
+// the launchers of the built instantiations, by n_half - 1
+constexpr Runner kRunV3[4]      = { launch_v3<1, false>, launch_v3<2, false>, launch_v3<3, false>, launch_v3<4, false> };
+constexpr Runner kRunV3Sym[3]   = { launch_v3<1, true>, launch_v3<2, true>, launch_v3<3, true> };
+constexpr Runner kRunV3Pre[3]   = { launch_v3_pre<1>, launch_v3_pre<2>, launch_v3_pre<3> };
+template <int RS>
+constexpr Runner kRunV3f[3]     = { launch_v3f<1, RS>, launch_v3f<2, RS>, launch_v3f<3, RS> };
+constexpr Runner kRunV3w[3]     = { launch_v3w<1>, launch_v3w<2>, launch_v3w<3> };
+constexpr Runner kRunFast16[3]  = { launch_fast16<1>, launch_fast16<2>, launch_fast16<3> };
+constexpr Runner kRunTiled8[4]  = { launch_tiled<uint8_t, 1>, launch_tiled<uint8_t, 2>, launch_tiled<uint8_t, 3>, launch_tiled<uint8_t, 4> };
+constexpr Runner kRunTiled16[4] = { launch_tiled<uint16_t, 1>, launch_tiled<uint16_t, 2>, launch_tiled<uint16_t, 3>, launch_tiled<uint16_t, 4> };
+
+// fits the tile: the tile kernels' halo holds the patch and search window, their tensor maps the frames; no prefilter
+bool fits_tile(const KernelParams &k)
+{
+    return !k.use_pre && k.n_half >= 1 && k.n_half <= 4 && k.n_half + k.r_half <= kHalo && k.nf <= kMaxTiledFrames;
+}
+
+// the saturating table lookup of the fp32-exact kernels gives the reference's weights (see kLutEntries)
+bool table_trick_ok(const KernelParams &k) { return k.wfact < 0.99f && k.wfact > 1e-5f; }
+
+// every displacement row of the range splits into group shapes the v3 kernels are built with (range 1 does not)
+bool range_splits(int r_half)
+{
+    for (int dx0 = -r_half; dx0 <= r_half; dx0 += kGroup)
+    {
+        const int ng = std::min(kGroup, r_half - dx0 + 1), ob = (12 + dx0) & 3;
+        if (!v3_group_known(ng, ob, kOrgNone)) return false;
+        if (dx0 <= 0 && dx0 + ng > 0 && !v3_group_known(ng, ob, -dx0)) return false;
+    }
+    return true;
+}
+
+// the fp32-exact tile kernels (v3, v3f, v3w, fast16) may take the plane: impl 0 or 2, it fits the tile and the table
+// trick is valid; 16-bit planes must hold 10-bit video and a patch of at most 7 (their fp32 patch-row sums stay exact)
+bool fp32_exact_ok(const hbcu_nlmeans_s *h, const KernelParams &k)
+{
+    return (h->impl == 0 || h->impl == 2) && fits_tile(k) && table_trick_ok(k) && (h->bps == 1 || (h->cfg.depth <= 10 && k.n_half <= 3));
+}
+
+// nlmeans_v3f_kernel takes a plane at range 3 with one or two frames (patch 3 .. 7, no prefilter) on top of what the
+// 8-bit v3 kernel needs.  More frames keep the accumulating kernel: each further frame would add nine running sums to
+// registers that are full.
+bool v3f_fits(const hbcu_nlmeans_s *h, const KernelParams &k)
+{
+    return h->v3_fused && k.r_half == 1 && k.nf <= 2 && k.n_half >= 1 && k.n_half <= 3 && !k.use_pre;
+}
+
+Runner v3f_runner(int rs, int n_half)
+{
+    if (rs == kV3FusedTaller.rs) return kRunV3f<kV3FusedTaller.rs>[n_half - 1];
+    if (rs == kV3FusedTall.rs) return kRunV3f<kV3FusedTall.rs>[n_half - 1];
+    return kRunV3f<kV3Fused.rs>[n_half - 1];
+}
+
+// range 3 in every plane of the launch: frame 0 runs as one symmetric march (V3Sym, nlmeans_v3.cuh), built for 12 x 10
+Runner v3_runner(int n_half, bool all_range3) { return all_range3 && n_half <= 3 ? kRunV3Sym[n_half - 1] : kRunV3[n_half - 1]; }
+
+// the kernel of a plane launched on its own; nullptr (error set) when impl 2 meets a plane the tiled kernel cannot take
+Runner plane_kernel(const hbcu_nlmeans_s *h, const KernelParams &k)
+{
+    if (h->bps == 1 && h->impl == 0 && k.use_pre && k.n_half >= 1 && k.n_half <= 3 && k.n_half + k.r_half <= kHalo &&
+        k.nf <= kMaxTiledFrames && table_trick_ok(k) && range_splits(k.r_half))
+        return kRunV3Pre[k.n_half - 1];
+    if (h->impl == 1 || !fits_tile(k))
+    {
+        if (h->impl == 2)
+        {
+            set_error("nlmeans: tiled kernel does not support n=%d r=%d", 2 * k.n_half + 1, 2 * k.r_half + 1);
+            return nullptr;
+        }
+        return h->bps == 1 ? launch_generic<uint8_t> : launch_generic<uint16_t>;
+    }
+    if (h->bps == 1 && fp32_exact_ok(h, k))
+    {
+        if (v3f_fits(h, k)) return v3f_runner(h->v3f_rs, k.n_half);
+        return range_splits(k.r_half) ? v3_runner(k.n_half, k.r_half == 1) : launch_generic<uint8_t>;
+    }
+    return h->bps == 1 ? kRunTiled8[k.n_half - 1] : kRunTiled16[k.n_half - 1];
+}
+
+// The kernel launches of one frame, in order, chosen from the handle (bit depth, impl, v3_fused, v3f_rs) and each active
+// plane's patch and search half-widths, frame count, prefilter and wfact.  All active planes share one launch when the
+// fp32-exact kernels take each of them with the same patch size: at 16 bits v3w (fast16 where a range does not split),
+// followed per plane by the integer tiled kernel that takes the frame only if a sample exceeds 10 bits; at 8 bits, with
+// two planes or more, v3f or v3 when every range splits.  Otherwise every plane has its own launch (plane_kernel).
+// Returns the number of launches written to out (at most 4), or -1.
+int select_kernels(const hbcu_nlmeans_s *h, const FramePlanes &fr, Launch *out)
+{
+    int act[3] = { 0, 0, 0 }, nact = 0;
+    for (int pl = 0; pl < 3; pl++)
+        if (fr.active[pl]) act[nact++] = pl;
+    const int nh = nact > 0 ? fr.k[act[0]].n_half : 0;
+    bool shared = nact > 0, splits = true, v3f = true, range3 = true;
+    for (int i = 0; i < nact; i++)
+    {
+        const KernelParams &k = fr.k[act[i]];
+        shared = shared && fp32_exact_ok(h, k) && k.n_half == nh;
+        splits = splits && range_splits(k.r_half);
+        v3f = v3f && v3f_fits(h, k);
+        range3 = range3 && k.r_half == 1;
+    }
+    int n = 0;
+    if (shared && h->bps == 2)
+    {
+        out[n++] = Launch{ splits ? kRunV3w[nh - 1] : kRunFast16[nh - 1], nact, { act[0], act[1], act[2] }, false };
+        for (int i = 0; i < nact; i++) out[n++] = Launch{ kRunTiled16[nh - 1], 1, { act[i] }, true };
+        return n;
+    }
+    if (shared && nact > 1 && splits)
+    {
+        out[n++] = Launch{ v3f ? v3f_runner(h->v3f_rs, nh) : v3_runner(nh, range3), nact, { act[0], act[1], act[2] }, false };
+        return n;
+    }
+    for (int i = 0; i < nact; i++)
+    {
+        const Runner run = plane_kernel(h, fr.k[act[i]]);
+        if (run == nullptr) return -1;
+        out[n++] = Launch{ run, 1, { act[i] }, false };
+    }
+    return n;
 }
 
 inline void trace(hbcu_nlmeans_s *h, int64_t index, int point, cudaStream_t st)
@@ -2080,9 +1453,8 @@ int run_filter(hbcu_nlmeans_s *h, int64_t index, int navail, int oslot, void *co
     const int pair = h->pool_used < (int)h->ev_pool.size() / 2 ? h->pool_used : -1;
     if (pair >= 0) HBCU_CHECK(cudaEventRecord(h->ev_pool[2 * pair], h->s_compute));
     trace(h, index, TR_KERNEL_BEGIN, h->s_compute);
-    KernelParams kps[3];
-    int slots[3][kMaxFrames];
-    bool active[3] = { false, false, false };
+    FramePlanes fr;
+    for (bool &a : fr.active) a = false;
     for (int pl = 0; pl < 3; pl++)
     {
         const hbcu_nlmeans_plane_t &pp = h->cfg.plane[pl];
@@ -2109,13 +1481,13 @@ int run_filter(hbcu_nlmeans_s *h, int64_t index, int navail, int oslot, void *co
             HBCU_CHECK(cudaGetLastError());
             continue;
         }
-        KernelParams &kp = kps[pl];
+        KernelParams &kp = fr.k[pl];
         memset(&kp, 0, sizeof(kp));
         kp.nf    = navail < pp.nframes ? navail : pp.nframes;
         for (int f = 0; f < kp.nf; f++)
         {
             const int slot = (int)((index + f) % h->ring);
-            slots[pl][f] = slot;
+            fr.slots[pl][f] = slot;
             kp.planes[f] = h->ring_mem[slot * 3 + pl];
             kp.pre[f]    = h->has_pre[pl] ? h->pre_mem[slot * 3 + pl] : h->ring_mem[slot * 3 + pl];
         }
@@ -2134,98 +1506,16 @@ int run_filter(hbcu_nlmeans_s *h, int64_t index, int navail, int oslot, void *co
         kp.diff_max = pp.diff_max;
         kp.origin_tune = pp.origin_tune;
         kp.exptable = h->d_exptable + pl * HBCU_NLMEANS_EXPSIZE;
-        active[pl] = true;
+        fr.active[pl] = true;
     }
-    // all active planes in one launch when they can share the fast 8-bit kernel instantiation
-    bool fused = h->impl == 0 || h->impl == 2;
-    int nact = 0, nh = -1;
-    for (int pl = 0; pl < 3; pl++) nact += active[pl] ? 1 : 0;
-    for (int pl = 0; pl < 3 && fused; pl++)
+    Launch plan[4];
+    const int nlaunch = select_kernels(h, fr, plan);
+    if (nlaunch < 0) return -1;
+    for (int i = 0; i < nlaunch; i++)
     {
-        if (!active[pl]) continue;
-        if (!fast8_ok(h, kps[pl])) fused = false;
-        if (nh < 0) nh = kps[pl].n_half; else if (nh != kps[pl].n_half) fused = false;
-    }
-    const int nh8 = nh;
-    bool fused16 = (h->impl == 0 || h->impl == 2) && h->bps == 2;
-    nh = -1;
-    for (int pl = 0; pl < 3 && fused16; pl++)
-    {
-        if (!active[pl]) continue;
-        if (!fast16_ok(h, kps[pl])) fused16 = false;
-        if (nh < 0) nh = kps[pl].n_half; else if (nh != kps[pl].n_half) fused16 = false;
-    }
-    if (fused16 && nact > 0)
-    {
-        FusedParams fp;
-        fp.nplanes = 0;
-        fp.range_flag = h->d_range_flag;
-        for (int pl = 0; pl < 3; pl++)
-        {
-            if (!active[pl]) continue;
-            fp.k[fp.nplanes] = kps[pl];
-            for (int f = 0; f < kps[pl].nf; f++) fp.maps[fp.nplanes][f] = (h->v3_nw > 0 ? h->maps3 : h->maps)[slots[pl][f] * 3 + pl];
-            fp.nplanes++;
-        }
-        int rc16 = h->v3_nw > 0 ? launch_v3w_nh(fp, h->s_compute) : 1;
-        if (rc16 > 0)
-        {
-            // a range the v3 group shapes do not cover (or v3 switched off): the round-1 kernel on its own tensor maps
-            fp.nplanes = 0;
-            for (int pl = 0; pl < 3; pl++)
-            {
-                if (!active[pl]) continue;
-                for (int f = 0; f < kps[pl].nf; f++) fp.maps[fp.nplanes][f] = h->maps[slots[pl][f] * 3 + pl];
-                fp.nplanes++;
-            }
-            rc16 = launch_fast16_nh(fp, h->s_compute);
-        }
-        if (rc16 != 0) { set_error("nlmeans: fused 16-bit launch failed"); return -1; }
+        if (plan[i].run(h, fr, plan[i]) != 0) return -1;
         HBCU_CHECK(cudaGetLastError());
-        h->kernel_launches++;
-        // stand-in for frames with samples above 10 bit: returns immediately unless the border kernel raised the flag
-        const int saved_impl = h->impl;
-        h->impl = 3;
-        for (int pl = 0; pl < 3; pl++)
-        {
-            if (!active[pl]) continue;
-            if (launch_plane(h, kps[pl], slots[pl], pl, h->d_range_flag) != 0) { h->impl = saved_impl; return -1; }
-        }
-        h->impl = saved_impl;
-    }
-    else if (fused && nact > 1)
-    {
-        FusedParams fp;
-        fp.nplanes = 0;
-        fp.range_flag = nullptr;
-        V3Shape vs;
-        const bool v3 = v3_pick(h, nh8, &vs);
-        const bool v3f = v3 && v3f_ok(h, kps, active, 3);
-        for (int pl = 0; pl < 3; pl++)
-        {
-            if (!active[pl]) continue;
-            fp.k[fp.nplanes] = kps[pl];
-            for (int f = 0; f < kps[pl].nf; f++) fp.maps[fp.nplanes][f] = (v3f ? h->maps3f : v3 ? h->maps3 : h->maps)[slots[pl][f] * 3 + pl];
-            fp.nplanes++;
-        }
-        const int rc8 = v3f ? launch_v3f_nh(h->v3f_rs, fp, h->s_compute) : v3 ? launch_v3_nh(vs.nw, vs.rs, fp, h->s_compute) : launch_fast8_nh(fp, h->s_compute);
-        if (rc8 < 0) { set_error("nlmeans: fused launch failed"); return -1; }
-        if (rc8 == 0)
-        {
-            HBCU_CHECK(cudaGetLastError());
-            h->kernel_launches++;
-        }
-        // a range the v3 group shapes do not cover (range 1): one launch per plane, as launch_plane() picks for it
-        else fused = false;
-    }
-    if (!(fused16 && nact > 0) && !(fused && nact > 1))
-    {
-        for (int pl = 0; pl < 3; pl++)
-        {
-            if (!active[pl]) continue;
-            if (launch_plane(h, kps[pl], slots[pl], pl) != 0) return -1;
-            h->kernel_launches++;
-        }
+        if (!plan[i].if_flag) h->kernel_launches++;
     }
     if (pair >= 0)
     {
@@ -2302,23 +1592,8 @@ int hbcu_nlmeans_create(hbcu_nlmeans_t **out, const hbcu_nlmeans_config_t *cfg)
     h->bps = cfg->depth > 8 ? 2 : 1;
     h->impl = 0;
     if (const char *e = getenv("HBCU_NLMEANS_IMPL")) h->impl = atoi(e) >= 0 && atoi(e) <= 3 ? atoi(e) : 0;   // test hook
-    if (const char *e = getenv("HBCU_NLMEANS_SSD")) g_ssd_variant = atoi(e);                                  // tuning hook
-    // v3 8-bit kernel shape; HBCU_NLMEANS_V3=off | "warps,rows" (tuning hook, see v3_shape_ok)
-    h->v3_nw = kV3Default.nw; h->v3_rs = kV3Default.rs;
-    if (const char *e = getenv("HBCU_NLMEANS_V3"))
-    {
-        int a = 0, b = 0;
-        if (sscanf(e, "%d,%d", &a, &b) == 2 && v3_shape_ok(a, b, 3)) { h->v3_nw = a; h->v3_rs = b; }
-        else h->v3_nw = 0;
-    }
-    if (h->bps != 1)
-    {
-        // 16-bit planes have one v3 shape (nlmeans_v3w_kernel); HBCU_NLMEANS_V3=off still selects the round-1 kernel
-        const bool off = h->v3_nw == 0;
-        h->v3_nw = off ? 0 : kV3wShape.nw; h->v3_rs = kV3wShape.rs;
-    }
     // range 3 with nf <= 2 on 8-bit planes: the one-march kernel; HBCU_NLMEANS_V3_FUSED=0 keeps the accumulating one (A/B hook)
-    h->v3_fused = h->bps == 1 && h->v3_nw == kV3Default.nw && h->v3_rs == kV3Default.rs;
+    h->v3_fused = h->bps == 1;
     if (const char *e = getenv("HBCU_NLMEANS_V3_FUSED")) h->v3_fused = h->v3_fused && atoi(e) != 0;
     h->ring = cfg->ring_frames > 0 ? cfg->ring_frames : 8;
     h->out_slots = cfg->out_slots > 0 ? cfg->out_slots : 4;
@@ -2434,10 +1709,9 @@ int hbcu_nlmeans_create(hbcu_nlmeans_t **out, const hbcu_nlmeans_config_t *cfg)
                 hbcu_nlmeans_destroy(h);
                 return -1;
             }
-            if (h->v3_nw > 0 &&
-                hbcu::encode_tensor_map_2d(&h->maps3[s * 3 + pl], h->bps, h->ring_mem[s * 3 + pl], (uint64_t)h->g[pl].bw,
+            if (hbcu::encode_tensor_map_2d(&h->maps3[s * 3 + pl], h->bps, h->ring_mem[s * 3 + pl], (uint64_t)h->g[pl].bw,
                                            (uint64_t)h->g[pl].bh, (uint64_t)h->g[pl].bpitch * h->bps, kTilePW,
-                                           v3_box_rows(h->v3_nw, h->v3_rs)) != 0)
+                                           v3_box_rows(kV3Default.nw, kV3Default.rs)) != 0)
             {
                 hbcu_nlmeans_destroy(h);
                 return -1;
@@ -2450,10 +1724,10 @@ int hbcu_nlmeans_create(hbcu_nlmeans_t **out, const hbcu_nlmeans_config_t *cfg)
                 hbcu_nlmeans_destroy(h);
                 return -1;
             }
-            if (h->v3_nw > 0 && h->has_pre[pl] &&
+            if (h->has_pre[pl] &&
                 hbcu::encode_tensor_map_2d(&h->maps3_pre[s * 3 + pl], h->bps, h->pre_mem[s * 3 + pl], (uint64_t)h->g[pl].bw,
                                            (uint64_t)h->g[pl].bh, (uint64_t)h->g[pl].bpitch * h->bps, kTilePW,
-                                           v3_box_rows(h->v3_nw, h->v3_rs)) != 0)
+                                           v3_box_rows(kV3Default.nw, kV3Default.rs)) != 0)
             {
                 hbcu_nlmeans_destroy(h);
                 return -1;

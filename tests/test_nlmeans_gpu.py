@@ -125,23 +125,19 @@ def test_golden_digests(cuda_filters):
         assert [hashlib.sha256(f.tobytes()).hexdigest() for f in g.frames] == c["sha256"], name
 
 
-@pytest.mark.parametrize("ssd", ["0", "1"])
-def test_both_ssd_formulations(ref, cuda_filters, monkeypatch, ssd):
-    """fp32-prefix-sum (0) and VABSDIFF4+IDP4A (1) patch-row sums, patch sizes 3/5/7/9 over the three planes"""
-    monkeypatch.setenv("HBCU_NLMEANS_SSD", ssd)
+@pytest.mark.parametrize("settings", ["y-strength=6:y-patch-size=7:cb-strength=5:cb-patch-size=5:cb-range=5:cr-patch-size=3",
+                                      "y-strength=8:y-patch-size=9:y-range=5:y-frame-count=3"], ids=["p7-p5-p3", "p9-r5"])
+def test_patch_sizes_across_planes(ref, cuda_filters, settings):
+    """patch sizes 3/5/7/9 over the three planes: per-plane launches, and patch 9 in the 8-warp v3 shape"""
     w, h = 300, 170
     clip = synth.progressive_clip(FMT8, w, h, 4, seed=23)
-    for s in ("y-strength=6:y-patch-size=7:cb-strength=5:cb-patch-size=5:cb-range=5:cr-patch-size=3",
-              "y-strength=8:y-patch-size=9:y-range=5:y-frame-count=3"):
-        r, g = run_both(ref, cuda_filters, s, clip, FMT8, w, h)
-        assert_same(r, g)
+    r, g = run_both(ref, cuda_filters, settings, clip, FMT8, w, h)
+    assert_same(r, g)
 
 
 @pytest.mark.parametrize("fmt", [FMT8, FMT10])
-def test_round1_kernels_still_agree(ref, cuda_filters, monkeypatch, fmt):
-    """HBCU_NLMEANS_V3=off selects the round-1 fused kernels (nlmeans_fast8 / fast16), the baseline of the v3 kernels:
-    they stay bit-exact"""
-    monkeypatch.setenv("HBCU_NLMEANS_V3", "off")
+def test_ragged_frame_range3_and_range5(ref, cuda_filters, fmt):
+    """a frame size that is no multiple of any tile, at range 3 (2 frames) and range 5 (3 frames), 8 and 10 bits"""
     w, h = 330, 210
     clip = synth.progressive_clip(fmt, w, h, 4, seed=33)
     for s in ("y-strength=6", "y-strength=10:y-patch-size=5:y-range=5:y-frame-count=3"):

@@ -1,11 +1,11 @@
 """NLMeans across its parameter space: search ranges 1-27, frame counts up to 32, patch sizes 1-31, the strengths at the
 limits of the fast kernels' table trick, 8/10/12-bit, the v3 prefilter variant and every shipping preset x tune.
 
-`run_filter` / `launch_plane` in handbrake_b200/csrc/nlmeans.cu choose between about ten kernels from the patch size,
-range, frame count, strength (through wfact), bit depth and prefilter of each plane, and from whether all planes fit
-one launch.  CASES names, for each job, the kernel class it is meant to reach; `test_dispatch_coverage` restates that
-choice in Python and checks every claim, and that the 8-bit and 10-bit cases that reach the v3 kernels run every group
-shape those kernels are built with (V3_GROUP_SHAPES in nlmeans_v3.cuh).
+`select_kernels` in handbrake_b200/csrc/nlmeans.cu chooses between about ten kernels from the patch size, range, frame
+count, strength (through wfact), bit depth and prefilter of each plane, and from whether all planes fit one launch.
+CASES names, for each job, the kernel class it is meant to reach; `test_dispatch_coverage` restates that choice in
+Python and checks every claim, and that the 8-bit and 10-bit cases that reach the v3 kernels run every group shape
+those kernels are built with (V3_GROUP_SHAPES in nlmeans_v3.cuh).
 
 Each case runs twice: without a GPU, the plain-C restatement (through the host filters) must reproduce the stored
 digest of the reference's result; on the GPU, hb_filter_nlmeans_cuda must reproduce the reference's frames bit for bit.
@@ -88,7 +88,7 @@ CLIPS = {"noise": clip_noise, "extreme": clip_extreme, "band": clip_band, "step"
 # ------------------------------------------------------------------------------------------------------------ cases
 Case = namedtuple("Case", "id settings fmt w h n clip cls threads")
 # clip: (kind, seed, *args) of CLIPS; cls: the kernel class the first output frame is meant to reach (dispatch())
-CLASSES = ("v3 fused", "v3 planes", "v3 pre", "fused fallback", "v3w fused", "fast16 fused", "tiled8", "tiled16", "generic")
+CLASSES = ("v3 fused", "v3 planes", "v3 pre", "v3w fused", "fast16 fused", "tiled8", "tiled16", "generic")
 
 
 def plane_settings(patch, rng, frames=2, strength=6, prefix="y"):
@@ -115,10 +115,8 @@ def _sweep():
     for patch in (3, 5, 7, 9):
         edge = _halo_edge(patch)
         for rng in range(1, edge + 3, 2):
-            if rng == 1:
-                cls = "fused fallback"
-            else:
-                cls = "v3 fused" if rng <= edge else "generic"
+            # range 1 splits into no v3 group shape: one generic launch per plane
+            cls = "v3 fused" if 1 < rng <= edge else "generic"
             out.append(case(f"sweep8-p{patch}-r{rng}", plane_settings(patch, rng), FMT8, G_WIDE if rng <= 7 else G_SMALL,
                             2, ("noise", 10 * patch + rng), cls))
     for patch in (3, 5, 7):
@@ -318,14 +316,14 @@ def v3_group_shapes():
 
 
 def v3_groups(r_half):
-    """launch_v3_nh: a displacement row cut into groups of K_GROUP, the remainder last -> (dx0, ng, (12 + dx0) & 3)"""
+    """range_splits: a displacement row cut into groups of K_GROUP, the remainder last -> (dx0, ng, (12 + dx0) & 3)"""
     for dx0 in range(-r_half, r_half + 1, K_GROUP):
         ng = min(K_GROUP, r_half - dx0 + 1)
         yield dx0, ng, (12 + dx0) & 3
 
 
 def v3_known(r_half, known):
-    """launch_v3_nh / launch_v3w_nh: every group of the range, and its origin variant, is a built shape"""
+    """range_splits: every group of the range, and its origin variant, is a built shape"""
     return all((ng, ob, None) in known and (not dx0 <= 0 < dx0 + ng or (ng, ob, -dx0) in known)
                for dx0, ng, ob in v3_groups(r_half))
 
@@ -379,8 +377,8 @@ def plane_params(settings, depth):
 
 
 def dispatch(c):
-    """the kernel class of the first output frame and the v3 / v3w group shapes it runs, as run_filter() and
-    launch_plane() choose them (default build: v3 on, 12 warps x 10 rows)"""
+    """the kernel class of the first output frame and the v3 / v3w group shapes it runs, as select_kernels() and
+    plane_kernel() choose them (HBCU_NLMEANS_IMPL unset)"""
     depth = synth.depth_of(c.fmt)
     params = plane_params(c.settings, depth)
     navail = min(max(p["frame-count"] for p in params), c.n)
@@ -404,12 +402,9 @@ def dispatch(c):
                 return "v3w fused", shapes
             return "fast16 fused", shapes
         return ("tiled16" if any(k["tiled"] for k in planes) else "generic"), shapes
-    fallback = False
-    if len(planes) > 1 and same_nh and all(k["tiled"] and k["window"] for k in planes):
-        if all(k["known"] for k in planes):
-            shapes["v3"] = v3_launch_shapes(planes, sym_ok=planes[0]["n_half"] <= 3)
-            return "v3 fused", shapes
-        fallback = True
+    if len(planes) > 1 and same_nh and all(k["tiled"] and k["window"] and k["known"] for k in planes):
+        shapes["v3"] = v3_launch_shapes(planes, sym_ok=planes[0]["n_half"] <= 3)
+        return "v3 fused", shapes
     kinds = set()
     for k in planes:
         if k["pre"] and 1 <= k["n_half"] <= 3 and k["n_half"] + k["r_half"] <= K_HALO and k["nf"] <= K_MAX_TILED_FRAMES \
@@ -422,8 +417,6 @@ def dispatch(c):
             kinds.add("tiled8")
         else:
             kinds.add("generic")
-    if fallback:
-        return "fused fallback", shapes
     return next(cls for cls in ("v3 pre", "v3 planes", "tiled8", "generic") if cls in kinds), shapes
 
 
