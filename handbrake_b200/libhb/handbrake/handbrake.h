@@ -132,6 +132,11 @@ const AVPixFmtDescriptor *av_pix_fmt_desc_get(int pix_fmt);
 int av_image_get_linesize(int pix_fmt, int width, int plane);
 /* number of distinct planes of the format (libavutil/pixdesc.c), < 0 for an unknown format */
 int av_pix_fmt_count_planes(int pix_fmt);
+/* libavutil/pixdesc.c: the format of a descriptor name (or of the name with the native-endian suffix "le" appended,
+ * so "p010" is p010le and "yuv420p10" is yuv420p10le), AV_PIX_FMT_NONE for a name the table does not know; and the
+ * descriptor name of a format, NULL for an unknown one */
+enum AVPixelFormat av_get_pix_fmt(const char *name);
+const char *av_get_pix_fmt_name(enum AVPixelFormat pix_fmt);
 
 typedef struct AVRational { int num; int den; } AVRational;
 typedef struct AVChannelLayout { int order; int nb_channels; uint64_t mask; void *opaque; } AVChannelLayout;

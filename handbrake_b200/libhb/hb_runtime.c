@@ -70,6 +70,29 @@ const AVPixFmtDescriptor *av_pix_fmt_desc_get(int pix_fmt)
     }
 }
 
+enum AVPixelFormat av_get_pix_fmt(const char *name)
+{
+    static const enum AVPixelFormat known[] = {
+        AV_PIX_FMT_YUV420P, AV_PIX_FMT_YUV422P, AV_PIX_FMT_YUV444P, AV_PIX_FMT_GRAY8, AV_PIX_FMT_YUV420P10LE,
+        AV_PIX_FMT_YUV422P10LE, AV_PIX_FMT_YUV444P10LE, AV_PIX_FMT_YUV420P12LE, AV_PIX_FMT_YUV420P16LE,
+        AV_PIX_FMT_YUVA420P, AV_PIX_FMT_YUVA422P, AV_PIX_FMT_YUVA444P, AV_PIX_FMT_NV12, AV_PIX_FMT_P010LE, AV_PIX_FMT_P016LE,
+    };
+    if (name == NULL) return AV_PIX_FMT_NONE;
+    char native[64];
+    snprintf(native, sizeof(native), "%sle", name);
+    for (int pass = 0; pass < 2; pass++)
+        for (size_t i = 0; i < sizeof(known) / sizeof(known[0]); i++)
+            if (strcmp(av_pix_fmt_desc_get(known[i])->name, pass == 0 ? name : native) == 0)
+                return known[i];
+    return AV_PIX_FMT_NONE;
+}
+
+const char *av_get_pix_fmt_name(enum AVPixelFormat pix_fmt)
+{
+    const AVPixFmtDescriptor *d = av_pix_fmt_desc_get(pix_fmt);
+    return d != NULL ? d->name : NULL;
+}
+
 int av_pix_fmt_count_planes(int pix_fmt)
 {
     const AVPixFmtDescriptor *d = av_pix_fmt_desc_get(pix_fmt);

@@ -550,6 +550,44 @@ int  hbcu_motion_metric_elapsed_ms(hbcu_motion_metric_t *h, float *ms);
 uint64_t hbcu_motion_metric_waits(void);
 uint64_t hbcu_motion_metric_launches(void);
 
+/* ------------------------------------------------------------------------- */
+/* format       replaces the avfilter graph libhb/format.c builds (format /    */
+/*              scale_cuda with format=<pix_fmt>) for the four lossless 4:2:0  */
+/*              repacks between NVDEC / NVENC's semi-planar frames and the     */
+/*              planar pipeline formats                                         */
+/* ------------------------------------------------------------------------- */
+/*   depth 8,  to_semi_planar 0:  nv12        -> yuv420p       (Cb/Cr pairs of plane 1 split into planes 1 and 2)
+ *   depth 8,  to_semi_planar 1:  yuv420p     -> nv12
+ *   depth 10, to_semi_planar 0:  p010le      -> yuv420p10le   (every sample v >> 6: the 6 padding bits are dropped)
+ *   depth 10, to_semi_planar 1:  yuv420p10le -> p010le        (every sample v << 6, kept to 16 bits)
+ * One kernel launch per frame covers every plane.  The semi-planar side has two planes: as a device frame its third
+ * plane is absent (0 rows of 0 bytes), as host planes planes[2] / strides[2] are not read. */
+typedef struct hbcu_format_config_s
+{
+    int width, height;                   /* luma geometry; chroma is (width + 1) / 2 x (height + 1) / 2 */
+    int depth;                           /* 8 or 10 */
+    int to_semi_planar;                  /* 0: semi-planar -> planar, 1: planar -> semi-planar */
+    int device;
+    int slots;                           /* conversions in flight */
+} hbcu_format_config_t;
+
+typedef struct hbcu_format_s hbcu_format_t;
+
+int  hbcu_format_create(hbcu_format_t **out, const hbcu_format_config_t *cfg);
+void hbcu_format_destroy(hbcu_format_t *h);
+/* one frame; either side may be a device frame (NULL = the host planes / strides of that side, any linesize at least a
+ * row long; a host source is copied to the device behind the call and must stay untouched until wait / poll reports the
+ * ticket done).  A device source is read in place at its own pitch (a decoder surface, hb_image_stride, ...) and recorded
+ * as one of its readers; nothing waits on the host.  Asynchronous; `ticket` for wait / poll. */
+int  hbcu_format_convert(hbcu_format_t *h, int64_t ticket,
+                         hbcu_frame_t *in_frame, const void *const in_planes[3], const int in_strides[3],
+                         hbcu_frame_t *out_frame, void *const out_planes[3], const int out_strides[3]);
+int  hbcu_format_wait(hbcu_format_t *h, int64_t ticket);
+int  hbcu_format_poll(hbcu_format_t *h, int64_t ticket);
+int  hbcu_format_sync(hbcu_format_t *h);
+int  hbcu_format_mark(hbcu_format_t *h, int which);
+int  hbcu_format_elapsed_ms(hbcu_format_t *h, float *ms);
+
 #ifdef __cplusplus
 }
 #endif

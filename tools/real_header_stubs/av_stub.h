@@ -20,6 +20,9 @@ int av_image_get_linesize(enum AVPixelFormat pix_fmt, int width, int plane);
 typedef struct AVComponentDescriptor { int plane, step, offset, shift, depth; } AVComponentDescriptor;
 typedef struct AVPixFmtDescriptor { const char *name; uint8_t nb_components, log2_chroma_w, log2_chroma_h; uint64_t flags; AVComponentDescriptor comp[4]; const char *alias; } AVPixFmtDescriptor;
 const AVPixFmtDescriptor *av_pix_fmt_desc_get(enum AVPixelFormat pix_fmt);
+int av_pix_fmt_count_planes(enum AVPixelFormat pix_fmt);
+enum AVPixelFormat av_get_pix_fmt(const char *name);
+const char *av_get_pix_fmt_name(enum AVPixelFormat pix_fmt);
 typedef struct AVChannelLayout { int order, nb_channels; union { uint64_t mask; void *map; } u; void *opaque; } AVChannelLayout;
 typedef struct AVBufferRef AVBufferRef;
 typedef struct AVFrame AVFrame;
