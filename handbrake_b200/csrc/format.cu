@@ -20,12 +20,12 @@
 // HBM bound: read one frame, write one frame.
 #include "hbcu_common.h"
 #include "hbcu_frames.h"
+#include "hbcu_staging.h"
 #include "../../include/hbcu.h"
 
 #include <cstdlib>
 #include <cstring>
 #include <new>
-#include <vector>
 
 namespace {
 
@@ -162,68 +162,18 @@ __global__ void __launch_bounds__(kThreads) format_kernel(const FormatArgs a)
     }
 }
 
-struct PlaneGeom { int row_bytes, rows, pitch; size_t off; };
-
 }  // namespace
 
 struct hbcu_format_s
 {
     hbcu_format_config_t cfg;
-    int bps, slots, next;
+    int bps;
     int cw, ch;
-    PlaneGeom in[3], out[3];                 // staging layout of each side (hb_image_stride pitches); in[2] / out[2] of the
-                                             // semi-planar side has 0 rows
-    size_t in_bytes, out_bytes;
-    std::vector<uint8_t *> in_stage, out_stage;    // per slot, allocated on first use by a host side
-    std::vector<int64_t> ticket;
-    cudaStream_t s_h2d, s_compute, s_d2h;
-    std::vector<cudaEvent_t> ev_up, ev_k, ev_down;
-    cudaEvent_t ev_mark[2];
+    hbcu::Staging st;                        // in / out: the two sides' planes; the third plane of the semi-planar side
+                                             // has 0 rows
 };
 
 namespace {
-
-// the planes of one side: semi-planar (Y, Cb/Cr pairs) or planar (Y, Cb, Cr); hb_image_stride pitches
-size_t side_layout(PlaneGeom g[3], bool semi, int w, int h, int cw, int ch, int bps)
-{
-    const int rb[3] = {w * bps, semi ? 2 * cw * bps : cw * bps, semi ? 0 : cw * bps};
-    const int rows[3] = {h, ch, semi ? 0 : ch};
-    size_t off = 0;
-    for (int p = 0; p < 3; p++)
-    {
-        g[p].row_bytes = rb[p];
-        g[p].rows = rows[p];
-        g[p].pitch = (rb[p] + 63) / 64 * 64;
-        g[p].off = off;
-        off += (size_t)g[p].pitch * rows[p];
-    }
-    return off;
-}
-
-bool frame_fits(const hbcu_format_s *h, const hbcu_frame_t *f, const PlaneGeom g[3])
-{
-    if (f->device != h->cfg.device) return false;
-    for (int p = 0; p < 3; p++)
-    {
-        if (f->rows[p] != g[p].rows || f->row_bytes[p] != g[p].row_bytes) return false;
-        if (g[p].rows > 0 && f->plane[p] == nullptr) return false;
-    }
-    return true;
-}
-
-bool host_fits(const void *const planes[3], const int strides[3], const PlaneGeom g[3])
-{
-    for (int p = 0; p < 3; p++)
-        if (g[p].rows > 0 && (planes[p] == nullptr || strides[p] < g[p].row_bytes)) return false;
-    return true;
-}
-
-int find_slot(const hbcu_format_s *h, int64_t ticket)
-{
-    for (int s = 0; s < h->slots; s++)
-        if (h->ticket[s] == ticket) return s;
-    return -1;
-}
 
 int launch(hbcu_format_s *h, const uint8_t *const src[3], const int spitch[3], uint8_t *const dst[3], const int dpitch[3])
 {
@@ -239,19 +189,28 @@ int launch(hbcu_format_s *h, const uint8_t *const src[3], const int spitch[3], u
     const int chunks = a.luma_chunks > a.chroma_chunks ? a.luma_chunks : a.chroma_chunks;
     const dim3 grid((chunks + kThreads - 1) / kThreads, a.h + a.ch);
     const bool semi = h->cfg.to_semi_planar != 0;
+    cudaStream_t st = h->st.s_compute;
     if (h->bps == 1)
     {
-        if (semi) format_kernel<uint8_t, 0, true><<<grid, kThreads, 0, h->s_compute>>>(a);
-        else      format_kernel<uint8_t, 0, false><<<grid, kThreads, 0, h->s_compute>>>(a);
+        if (semi) format_kernel<uint8_t, 0, true><<<grid, kThreads, 0, st>>>(a);
+        else      format_kernel<uint8_t, 0, false><<<grid, kThreads, 0, st>>>(a);
     }
     else
     {
-        if (semi) format_kernel<uint16_t, 6, true><<<grid, kThreads, 0, h->s_compute>>>(a);
-        else      format_kernel<uint16_t, 6, false><<<grid, kThreads, 0, h->s_compute>>>(a);
+        if (semi) format_kernel<uint16_t, 6, true><<<grid, kThreads, 0, st>>>(a);
+        else      format_kernel<uint16_t, 6, false><<<grid, kThreads, 0, st>>>(a);
     }
     hbcu::count_launch();
     HBCU_CHECK(cudaGetLastError());
     return 0;
+}
+
+// the planes of one side: semi-planar (Y, Cb/Cr pairs) or planar (Y, Cb, Cr)
+size_t side_layout(hbcu::StagePlane g[3], bool semi, int w, int h, int cw, int ch, int bps)
+{
+    const int rb[3] = {w * bps, semi ? 2 * cw * bps : cw * bps, semi ? 0 : cw * bps};
+    const int rows[3] = {h, ch, semi ? 0 : ch};
+    return hbcu::stage_layout(g, rb, rows);
 }
 
 }  // namespace
@@ -289,42 +248,16 @@ int hbcu_format_create(hbcu_format_t **out, const hbcu_format_config_t *cfg)
     if (h == nullptr) { set_error("format_create: out of memory"); return -1; }
     h->cfg = *cfg;
     h->bps = cfg->depth > 8 ? 2 : 1;
-    h->slots = cfg->slots >= 2 ? cfg->slots : 4;
-    h->next = 0;
     h->cw = (cfg->width + 1) >> 1;
     h->ch = ch;
     const bool to_semi = cfg->to_semi_planar != 0;
-    h->in_bytes = side_layout(h->in, !to_semi, cfg->width, cfg->height, h->cw, h->ch, h->bps);
-    h->out_bytes = side_layout(h->out, to_semi, cfg->width, cfg->height, h->cw, h->ch, h->bps);
-    h->s_h2d = h->s_compute = h->s_d2h = nullptr;
-    h->ev_mark[0] = h->ev_mark[1] = nullptr;
-#define CK(expr)                                                                  \
-    do {                                                                          \
-        cudaError_t _e = (expr);                                                  \
-        if (_e != cudaSuccess) {                                                  \
-            set_error("%s failed: %s", #expr, cudaGetErrorString(_e));            \
-            hbcu_format_destroy(h);                                               \
-            return -1;                                                            \
-        }                                                                         \
-    } while (0)
-    CK(cudaStreamCreateWithFlags(&h->s_h2d, cudaStreamNonBlocking));
-    CK(cudaStreamCreateWithFlags(&h->s_compute, cudaStreamNonBlocking));
-    CK(cudaStreamCreateWithFlags(&h->s_d2h, cudaStreamNonBlocking));
-    h->in_stage.assign(h->slots, nullptr);
-    h->out_stage.assign(h->slots, nullptr);
-    h->ticket.assign(h->slots, -1);
-    h->ev_up.assign(h->slots, nullptr);
-    h->ev_k.assign(h->slots, nullptr);
-    h->ev_down.assign(h->slots, nullptr);
-    for (int s = 0; s < h->slots; s++)
+    h->st.in_bytes = side_layout(h->st.in, !to_semi, cfg->width, cfg->height, h->cw, h->ch, h->bps);
+    h->st.out_bytes = side_layout(h->st.out, to_semi, cfg->width, cfg->height, h->cw, h->ch, h->bps);
+    if (hbcu::stage_init(&h->st, "format", cfg->device, cfg->slots >= 2 ? cfg->slots : 4) != 0)
     {
-        CK(cudaEventCreateWithFlags(&h->ev_up[s], cudaEventDisableTiming));
-        CK(cudaEventCreateWithFlags(&h->ev_k[s], cudaEventDisableTiming));
-        CK(cudaEventCreateWithFlags(&h->ev_down[s], cudaEventDisableTiming));
+        hbcu_format_destroy(h);
+        return -1;
     }
-    CK(cudaEventCreate(&h->ev_mark[0]));
-    CK(cudaEventCreate(&h->ev_mark[1]));
-#undef CK
     *out = h;
     return 0;
 }
@@ -332,20 +265,7 @@ int hbcu_format_create(hbcu_format_t **out, const hbcu_format_config_t *cfg)
 void hbcu_format_destroy(hbcu_format_t *h)
 {
     if (h == nullptr) return;
-    cudaSetDevice(h->cfg.device);
-    if (h->s_h2d) cudaStreamSynchronize(h->s_h2d);
-    if (h->s_compute) cudaStreamSynchronize(h->s_compute);
-    if (h->s_d2h) cudaStreamSynchronize(h->s_d2h);
-    for (auto p : h->in_stage) if (p) cudaFree(p);
-    for (auto p : h->out_stage) if (p) cudaFree(p);
-    for (auto e : h->ev_up) if (e) cudaEventDestroy(e);
-    for (auto e : h->ev_k) if (e) cudaEventDestroy(e);
-    for (auto e : h->ev_down) if (e) cudaEventDestroy(e);
-    if (h->ev_mark[0]) cudaEventDestroy(h->ev_mark[0]);
-    if (h->ev_mark[1]) cudaEventDestroy(h->ev_mark[1]);
-    if (h->s_h2d) cudaStreamDestroy(h->s_h2d);
-    if (h->s_compute) cudaStreamDestroy(h->s_compute);
-    if (h->s_d2h) cudaStreamDestroy(h->s_d2h);
+    hbcu::stage_destroy(&h->st);
     delete h;
 }
 
@@ -353,123 +273,40 @@ int hbcu_format_convert(hbcu_format_t *h, int64_t ticket,
                         hbcu_frame_t *in_frame, const void *const in_planes[3], const int in_strides[3],
                         hbcu_frame_t *out_frame, void *const out_planes[3], const int out_strides[3])
 {
-    if (h == nullptr || (in_frame == nullptr && (in_planes == nullptr || in_strides == nullptr)) ||
-        (out_frame == nullptr && (out_planes == nullptr || out_strides == nullptr)))
-    {
-        set_error("format_convert: bad argument");
-        return -1;
-    }
-    if ((in_frame ? !frame_fits(h, in_frame, h->in) : !host_fits(in_planes, in_strides, h->in)) ||
-        (out_frame ? !frame_fits(h, out_frame, h->out) : !host_fits(out_planes, out_strides, h->out)))
-    {
-        set_error("format_convert: a frame's planes do not match the handle's geometry and formats");
-        return -1;
-    }
-    HBCU_CHECK(cudaSetDevice(h->cfg.device));
-    const int s = h->next;
-    const uint8_t *src[3];
-    uint8_t *dst[3];
-    int spitch[3], dpitch[3];
-    if (in_frame == nullptr)
-    {
-        if (h->in_stage[s] == nullptr) HBCU_CHECK(cudaMalloc(&h->in_stage[s], h->in_bytes));
-        // the slot's previous kernel has read the staging
-        HBCU_CHECK(cudaStreamWaitEvent(h->s_h2d, h->ev_k[s], 0));
-        for (int p = 0; p < 3; p++)
-        {
-            src[p] = h->in_stage[s] + h->in[p].off;
-            spitch[p] = h->in[p].pitch;
-            if (h->in[p].rows > 0)
-                HBCU_CHECK(cudaMemcpy2DAsync(h->in_stage[s] + h->in[p].off, (size_t)h->in[p].pitch, in_planes[p], (size_t)in_strides[p],
-                                             (size_t)h->in[p].row_bytes, (size_t)h->in[p].rows, cudaMemcpyHostToDevice, h->s_h2d));
-        }
-        HBCU_CHECK(cudaEventRecord(h->ev_up[s], h->s_h2d));
-        HBCU_CHECK(cudaStreamWaitEvent(h->s_compute, h->ev_up[s], 0));
-    }
-    else
-    {
-        for (int p = 0; p < 3; p++) { src[p] = in_frame->plane[p]; spitch[p] = in_frame->stride[p]; }
-        if (hbcu::frame_begin_read(in_frame, h->s_compute) != 0) return -1;
-    }
-    if (out_frame == nullptr)
-    {
-        if (h->out_stage[s] == nullptr) HBCU_CHECK(cudaMalloc(&h->out_stage[s], h->out_bytes));
-        for (int p = 0; p < 3; p++) { dst[p] = h->out_stage[s] + h->out[p].off; dpitch[p] = h->out[p].pitch; }
-        HBCU_CHECK(cudaStreamWaitEvent(h->s_compute, h->ev_down[s], 0));     // the slot's previous copy-out is done
-    }
-    else
-    {
-        for (int p = 0; p < 3; p++) { dst[p] = out_frame->plane[p]; dpitch[p] = out_frame->stride[p]; }
-        if (hbcu::frame_begin_write(out_frame, h->s_compute) != 0) return -1;
-    }
-    h->next = (h->next + 1) % h->slots;
-    h->ticket[s] = -1;
-    if (launch(h, src, spitch, dst, dpitch) != 0) return -1;
-    HBCU_CHECK(cudaEventRecord(h->ev_k[s], h->s_compute));
-    if (in_frame && hbcu::frame_end_read(in_frame, h->s_compute) != 0) return -1;
-    if (out_frame)
-    {
-        if (hbcu::frame_end_write(out_frame, h->s_compute) != 0) return -1;
-        HBCU_CHECK(cudaEventRecord(h->ev_down[s], h->s_compute));
-    }
-    else
-    {
-        HBCU_CHECK(cudaStreamWaitEvent(h->s_d2h, h->ev_k[s], 0));
-        for (int p = 0; p < 3; p++)
-            if (h->out[p].rows > 0)
-                HBCU_CHECK(cudaMemcpy2DAsync(out_planes[p], (size_t)out_strides[p], dst[p], (size_t)dpitch[p],
-                                             (size_t)h->out[p].row_bytes, (size_t)h->out[p].rows, cudaMemcpyDeviceToHost, h->s_d2h));
-        HBCU_CHECK(cudaEventRecord(h->ev_down[s], h->s_d2h));
-    }
-    h->ticket[s] = ticket;
-    return 0;
+    if (h == nullptr) { set_error("format_convert: bad argument"); return -1; }
+    return hbcu::stage_submit(&h->st, "convert", ticket, in_frame, in_planes, in_strides, out_frame, out_planes, out_strides,
+                              [h](const uint8_t *const src[3], const int spitch[3], uint8_t *const dst[3], const int dpitch[3])
+                              { return launch(h, src, spitch, dst, dpitch); });
 }
 
 int hbcu_format_wait(hbcu_format_t *h, int64_t ticket)
 {
     if (h == nullptr) { set_error("format_wait: null handle"); return -1; }
-    const int s = find_slot(h, ticket);
-    if (s < 0) { set_error("format_wait: ticket %lld is not in flight", (long long)ticket); return -1; }
-    HBCU_CHECK(cudaEventSynchronize(h->ev_down[s]));
-    return 0;
+    return hbcu::stage_wait(&h->st, ticket);
 }
 
 int hbcu_format_poll(hbcu_format_t *h, int64_t ticket)
 {
     if (h == nullptr) { set_error("format_poll: null handle"); return -1; }
-    const int s = find_slot(h, ticket);
-    if (s < 0) { set_error("format_poll: ticket %lld is not in flight", (long long)ticket); return -1; }
-    cudaError_t e = cudaEventQuery(h->ev_down[s]);
-    if (e == cudaSuccess) return 1;
-    if (e == cudaErrorNotReady) return 0;
-    set_error("format_poll: %s", cudaGetErrorString(e));
-    return -1;
+    return hbcu::stage_poll(&h->st, ticket);
 }
 
 int hbcu_format_sync(hbcu_format_t *h)
 {
     if (h == nullptr) { set_error("format_sync: null handle"); return -1; }
-    HBCU_CHECK(cudaSetDevice(h->cfg.device));
-    HBCU_CHECK(cudaStreamSynchronize(h->s_h2d));
-    HBCU_CHECK(cudaStreamSynchronize(h->s_compute));
-    HBCU_CHECK(cudaStreamSynchronize(h->s_d2h));
-    return 0;
+    return hbcu::stage_sync(&h->st);
 }
 
 int hbcu_format_mark(hbcu_format_t *h, int which)
 {
     if (h == nullptr || which < 0 || which > 1) { set_error("format_mark: bad argument"); return -1; }
-    HBCU_CHECK(cudaSetDevice(h->cfg.device));
-    HBCU_CHECK(cudaEventRecord(h->ev_mark[which], h->s_compute));
-    return 0;
+    return hbcu::stage_mark(&h->st, which);
 }
 
 int hbcu_format_elapsed_ms(hbcu_format_t *h, float *ms)
 {
     if (h == nullptr || ms == nullptr) { set_error("format_elapsed_ms: bad argument"); return -1; }
-    HBCU_CHECK(cudaEventSynchronize(h->ev_mark[1]));
-    HBCU_CHECK(cudaEventElapsedTime(ms, h->ev_mark[0], h->ev_mark[1]));
-    return 0;
+    return hbcu::stage_elapsed_ms(&h->st, ms);
 }
 
 }  // extern "C"

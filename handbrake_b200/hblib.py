@@ -23,6 +23,8 @@ class HarnessIO(C.Structure):
         ("in_start", C.c_void_p), ("in_stop", C.c_void_p), ("in_new_chap", C.c_void_p),
         ("vrate_num", C.c_int), ("vrate_den", C.c_int), ("cfr", C.c_int), ("collect_info", C.c_int),
         ("out_new_chap", C.c_void_p), ("cfr_out", C.c_int), ("info_text", C.c_char * 128),
+        ("par_num", C.c_int), ("par_den", C.c_int),
+        ("par_num_out", C.c_int), ("par_den_out", C.c_int), ("width_out", C.c_int), ("height_out", C.c_int),
     ]
 
 
@@ -57,6 +59,8 @@ class FilterResult:
         self.new_chap = None
         self.cfr = 0
         self.info = ""
+        self.width = self.height = 0          # the output geometry and PAR (init->geometry after every init())
+        self.par = (1, 1)
 
 
 class FilterLib:
@@ -109,11 +113,12 @@ class FilterLib:
         self.lib.hb_shim_set_cpu_count(int(n))
 
     def run(self, filters, settings, frames, pix_fmt, width, height, flags=None, combed=None,
-            max_out=None, out_scale=1, start=None, stop=None, new_chap=None, vrate=None, cfr=0, info=False):
+            max_out=None, out_scale=1, start=None, stop=None, new_chap=None, vrate=None, cfr=0, info=False, par=None):
         """filters: list of exported object names; settings: list of 'k=v:k=v' strings (or None).
         frames: (n, frame_bytes) uint8 array.  start / stop / new_chap: per-frame input times and chapter marks
         (default i*3003, (i+1)*3003, i); vrate: (num, den) of the input (default 30000/1001); cfr: init->cfr;
-        info: fill FilterResult.info with the last info() text.  Returns FilterResult."""
+        info: fill FilterResult.info with the last info() text; par: (num, den) of the input (default 1:1).
+        Returns FilterResult, whose width / height / par are the output's."""
         if isinstance(filters, str):
             filters, settings = [filters], [settings]
         frames = np.ascontiguousarray(frames, dtype=np.uint8)
@@ -145,6 +150,8 @@ class FilterLib:
         if vrate is not None:
             io.vrate_num, io.vrate_den = int(vrate[0]), int(vrate[1])
         io.cfr, io.collect_info = int(cfr), int(bool(info))
+        if par is not None:
+            io.par_num, io.par_den = int(par[0]), int(par[1])
         o_chap = np.zeros(cap, dtype=np.int32)
         io.out_new_chap = o_chap.ctypes.data
         io.out, io.out_capacity = out.ctypes.data, cap
@@ -163,4 +170,5 @@ class FilterLib:
         r.saw_eof, r.init_failed = bool(io.saw_eof), io.init_failed
         r.vrate, r.n_dropped = (io.vrate_num_out, io.vrate_den_out), io.n_dropped
         r.new_chap, r.cfr, r.info = o_chap[:k], io.cfr_out, io.info_text.decode()
+        r.width, r.height, r.par = io.width_out, io.height_out, (io.par_num_out, io.par_den_out)
         return r

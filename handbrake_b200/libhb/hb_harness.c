@@ -155,8 +155,8 @@ int hb_harness_run_chain(int n_filters, hb_filter_object_t *const *protos,
     init.pix_fmt         = io->pix_fmt;
     init.geometry.width  = io->width;
     init.geometry.height = io->height;
-    init.geometry.par.num = 1;
-    init.geometry.par.den = 1;
+    init.geometry.par.num = io->par_num > 0 ? io->par_num : 1;
+    init.geometry.par.den = io->par_num > 0 ? io->par_den : 1;
     init.vrate.num = io->vrate_num > 0 ? io->vrate_num : 30000;
     init.vrate.den = io->vrate_den > 0 ? io->vrate_den : 1001;
     init.cfr       = io->cfr;
@@ -196,6 +196,10 @@ int hb_harness_run_chain(int n_filters, hb_filter_object_t *const *protos,
     io->vrate_num_out = init.vrate.num;
     io->vrate_den_out = init.vrate.den;
     io->cfr_out       = init.cfr;
+    io->par_num_out   = init.geometry.par.num;
+    io->par_den_out   = init.geometry.par.den;
+    io->width_out     = init.geometry.width;
+    io->height_out    = init.geometry.height;
     io->info_text[0]  = '\0';
     for (int k = 0; k < c.n && io->collect_info; k++)
     {

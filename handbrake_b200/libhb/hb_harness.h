@@ -38,6 +38,11 @@ typedef struct hb_harness_io_s
     int            *out_new_chap;
     int             cfr_out;     /* init->cfr after every filter's init() */
     char            info_text[128];   /* human_readable_desc of the last filter whose info() gives one */
+    /* input, optional: init->geometry.par (0 / 0: 1:1) */
+    int             par_num, par_den;
+    /* output: init->geometry after every filter's init() (the geometry of the frames in `out`) */
+    int             par_num_out, par_den_out;
+    int             width_out, height_out;
 } hb_harness_io_t;
 
 size_t       hb_harness_frame_bytes(int pix_fmt, int w, int h);

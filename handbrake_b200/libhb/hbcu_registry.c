@@ -15,6 +15,7 @@ extern hb_filter_object_t hb_filter_chroma_smooth_cuda;
 extern hb_filter_object_t hb_filter_detelecine_cuda;
 extern hb_filter_object_t hb_filter_vfr_cuda;
 extern hb_filter_object_t hb_filter_format_cuda;
+extern hb_filter_object_t hb_filter_rotate_cuda;
 
 hb_filter_object_t *hb_filter_get(int filter_id)
 {
@@ -30,6 +31,7 @@ hb_filter_object_t *hb_filter_get(int filter_id)
         case HB_FILTER_DETELECINE:  return &hb_filter_detelecine_cuda;    /* pullup: metrics on the device, decisions on the host */
         case HB_FILTER_VFR:         return &hb_filter_vfr_cuda;           /* motion metric on the device, read only when a drop is due */
         case HB_FILTER_FORMAT:      return &hb_filter_format_cuda;        /* nv12 / p010le <-> planar; init fails for other pairs */
+        case HB_FILTER_ROTATE:      return &hb_filter_rotate_cuda;        /* flips and transposes; init fails for 4:2:2 transposes */
         default:                return NULL;
     }
 }

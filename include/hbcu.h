@@ -588,6 +588,61 @@ int  hbcu_format_sync(hbcu_format_t *h);
 int  hbcu_format_mark(hbcu_format_t *h, int which);
 int  hbcu_format_elapsed_ms(hbcu_format_t *h, float *ms);
 
+/* ------------------------------------------------------------------------- */
+/* rotate       replaces the avfilter graph libhb/rotate.c builds (hflip /     */
+/*              vflip / transpose) for every planar and semi-planar format     */
+/*              whose planes transpose on their own                             */
+/* ------------------------------------------------------------------------- */
+/* Each plane is permuted within its own size.  An element is one sample of a planar plane or one Cb/Cr pair of a
+ * semi-planar chroma plane (it moves as one unit); for an input plane of pw x ph elements, output element (x, y) is
+ *   HBCU_ROTATE_HFLIP        in[y][pw-1-x]            (hflip; angle=0:hflip=1)
+ *   HBCU_ROTATE_VFLIP        in[ph-1-y][x]            (vflip; angle=180:hflip=1)
+ *   HBCU_ROTATE_180          in[ph-1-y][pw-1-x]       (vflip, hflip; angle=180:hflip=0)
+ *   HBCU_ROTATE_CLOCK        in[ph-1-x][y]            (transpose=clock; angle=90)            output ph x pw
+ *   HBCU_ROTATE_CLOCK_FLIP   in[ph-1-x][pw-1-y]       (transpose=clock_flip; angle=90:hflip=1)
+ *   HBCU_ROTATE_CCLOCK       in[x][pw-1-y]            (transpose=cclock; angle=270)
+ *   HBCU_ROTATE_CCLOCK_FLIP  in[x][y]                 (transpose=cclock_flip; angle=270:hflip=1)
+ * One kernel launch per frame covers every plane. */
+enum
+{
+    HBCU_ROTATE_HFLIP = 1,
+    HBCU_ROTATE_VFLIP,
+    HBCU_ROTATE_180,
+    HBCU_ROTATE_CLOCK,
+    HBCU_ROTATE_CLOCK_FLIP,
+    HBCU_ROTATE_CCLOCK,
+    HBCU_ROTATE_CCLOCK_FLIP,
+};
+
+typedef struct hbcu_rotate_config_s
+{
+    int planes;                          /* 3 planar, 2 semi-planar (Y, Cb/Cr pairs) */
+    int width[3], height[3];             /* each input plane in elements (hb_image_width / hb_image_height) */
+    int elem_bytes[3];                   /* bytes of one element: luma / chroma 1 / 1 (8-bit planar), 2 / 2 (9-16-bit
+                                          * planar), 1 / 2 (NV12), 2 / 4 (P010, P016) */
+    int transform;                       /* HBCU_ROTATE_* */
+    int device;
+    int slots;                           /* frames in flight */
+} hbcu_rotate_config_t;
+
+typedef struct hbcu_rotate_s hbcu_rotate_t;
+
+int  hbcu_rotate_create(hbcu_rotate_t **out, const hbcu_rotate_config_t *cfg);
+void hbcu_rotate_destroy(hbcu_rotate_t *h);
+/* one frame; either side may be a device frame (NULL = the host planes / strides of that side, any linesize at least a
+ * row long; a host source is copied to the device behind the call and must stay untouched until wait / poll reports the
+ * ticket done).  A device source is read in place at its own pitch and recorded as one of its readers.  The output
+ * planes have the transformed sizes (width and height swapped by the four transposes).  A semi-planar side's third
+ * plane is absent.  Asynchronous; `ticket` for wait / poll. */
+int  hbcu_rotate_frame(hbcu_rotate_t *h, int64_t ticket,
+                       hbcu_frame_t *in_frame, const void *const in_planes[3], const int in_strides[3],
+                       hbcu_frame_t *out_frame, void *const out_planes[3], const int out_strides[3]);
+int  hbcu_rotate_wait(hbcu_rotate_t *h, int64_t ticket);
+int  hbcu_rotate_poll(hbcu_rotate_t *h, int64_t ticket);
+int  hbcu_rotate_sync(hbcu_rotate_t *h);
+int  hbcu_rotate_mark(hbcu_rotate_t *h, int which);
+int  hbcu_rotate_elapsed_ms(hbcu_rotate_t *h, float *ms);
+
 #ifdef __cplusplus
 }
 #endif
