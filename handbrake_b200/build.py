@@ -26,9 +26,9 @@ NVCC_FLAGS = [
     "-Xcompiler", "-fPIC",
     "--expt-relaxed-constexpr",
 ]
-CU_SOURCES = ["hbcu_core.cu", "hbcu_frames.cu", "nlmeans.cu", "comb_detect.cu", "decomb.cu", "eedi2.cu", "lapsharp.cu", "unsharp.cu", "hqdn3d.cu", "detelecine.cu", "blend.cu", "motion_metric.cu", "format.cu", "rotate.cu"]
+CU_SOURCES = ["hbcu_core.cu", "hbcu_frames.cu", "nlmeans.cu", "comb_detect.cu", "decomb.cu", "eedi2.cu", "lapsharp.cu", "unsharp.cu", "hqdn3d.cu", "detelecine.cu", "blend.cu", "motion_metric.cu", "format.cu", "rotate.cu", "deinterlace.cu"]
 SHIM_SOURCES = ["hb_runtime.c", "hb_harness.c", "hb_bench.c"]
-C_SOURCES = ["hbcu_registry.c", "hbcu_pinned.c", "hbcu_device_frames.c", "nlmeans_cuda.c", "comb_detect_cuda.c", "decomb_cuda.c", "lapsharp_cuda.c", "unsharp_cuda.c", "denoise_cuda.c", "detelecine_cuda.c", "blend_cuda.c", "vfr_cuda.c", "format_cuda.c", "rotate_cuda.c"]
+C_SOURCES = ["hbcu_registry.c", "hbcu_pinned.c", "hbcu_device_frames.c", "nlmeans_cuda.c", "comb_detect_cuda.c", "decomb_cuda.c", "lapsharp_cuda.c", "unsharp_cuda.c", "denoise_cuda.c", "detelecine_cuda.c", "blend_cuda.c", "vfr_cuda.c", "format_cuda.c", "rotate_cuda.c", "deinterlace_cuda.c"]
 CFLAGS = ["-O2", "-std=gnu99", "-fPIC", "-Wall", "-Wno-unused-function", "-D__LIBHB__", "-pthread"]
 
 

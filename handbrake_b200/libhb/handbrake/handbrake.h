@@ -128,6 +128,10 @@ typedef struct AVPixFmtDescriptor
     AVComponentDescriptor comp[4];
 } AVPixFmtDescriptor;
 
+/* AVPixFmtDescriptor.flags bits (libavutil/pixdesc.h) */
+#define AV_PIX_FMT_FLAG_BE  (1 << 0)
+#define AV_PIX_FMT_FLAG_RGB (1 << 5)
+
 const AVPixFmtDescriptor *av_pix_fmt_desc_get(int pix_fmt);
 int av_image_get_linesize(int pix_fmt, int width, int plane);
 /* number of distinct planes of the format (libavutil/pixdesc.c), < 0 for an unknown format */

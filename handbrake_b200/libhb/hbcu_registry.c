@@ -16,6 +16,8 @@ extern hb_filter_object_t hb_filter_detelecine_cuda;
 extern hb_filter_object_t hb_filter_vfr_cuda;
 extern hb_filter_object_t hb_filter_format_cuda;
 extern hb_filter_object_t hb_filter_rotate_cuda;
+extern hb_filter_object_t hb_filter_yadif_cuda;
+extern hb_filter_object_t hb_filter_bwdif_cuda;
 
 hb_filter_object_t *hb_filter_get(int filter_id)
 {
@@ -32,6 +34,8 @@ hb_filter_object_t *hb_filter_get(int filter_id)
         case HB_FILTER_VFR:         return &hb_filter_vfr_cuda;           /* motion metric on the device, read only when a drop is due */
         case HB_FILTER_FORMAT:      return &hb_filter_format_cuda;        /* nv12 / p010le <-> planar; init fails for other pairs */
         case HB_FILTER_ROTATE:      return &hb_filter_rotate_cuda;        /* flips and transposes; init fails for 4:2:2 transposes */
+        case HB_FILTER_YADIF:       return &hb_filter_yadif_cuda;         /* init fails for semi-planar, gray and YUVA input */
+        case HB_FILTER_BWDIF:       return &hb_filter_bwdif_cuda;
         default:                return NULL;
     }
 }

@@ -643,6 +643,46 @@ int  hbcu_rotate_sync(hbcu_rotate_t *h);
 int  hbcu_rotate_mark(hbcu_rotate_t *h, int which);
 int  hbcu_rotate_elapsed_ms(hbcu_rotate_t *h, float *ms);
 
+/* ------------------------------------------------------------------------- */
+/* deinterlace  replaces the avfilter graphs libhb/deinterlace.c builds         */
+/*              (FFmpeg's yadif and bwdif) for planar 3-plane YUV               */
+/* ------------------------------------------------------------------------- */
+/* One picture is one field rebuilt from three frames: rows with ((y ^ parity) & 1) == 0 are copied from cur, the others
+ * are interpolated; p = parity ^ tff picks the neighbouring fields (prev2, next2) = p ? (prev, cur) : (cur, next).  The
+ * per-sample arithmetic of both algorithms is written out in DESIGN.md 4.9.  Each plane is filtered on its own with
+ * max = (1 << depth) - 1.  One kernel launch per call covers every plane and writes one or two pictures (both fields of
+ * a frame, in field mode); it reads each source row once for both. */
+enum
+{
+    HBCU_DEINT_YADIF = 1,
+    HBCU_DEINT_BWDIF = 2,
+};
+
+typedef struct hbcu_deint_config_s
+{
+    int algorithm;                       /* HBCU_DEINT_YADIF / HBCU_DEINT_BWDIF */
+    int width[3], height[3];             /* each plane in samples (hb_image_width / hb_image_height) */
+    int sample_bytes;                    /* 1 (8-bit) or 2 (9-16-bit, little-endian) */
+    int depth;                           /* bits per sample: the clip range, and Bwdif's row step (1 at 8 bits, else 2) */
+    int device;
+} hbcu_deint_config_t;
+
+typedef struct hbcu_deint_s hbcu_deint_t;
+
+int  hbcu_deint_create(hbcu_deint_t **out, const hbcu_deint_config_t *cfg);
+void hbcu_deint_destroy(hbcu_deint_t *h);
+/* pictures 0 .. npictures-1 (1 or 2) of frame `cur` into out[k], with parity[k] and, for Bwdif, intra[k] (the intra-only
+ * rule of the first and last picture of a stream); `spatial` turns on Yadif's spatial interlacing check (Bwdif always
+ * runs its own).  Every side is a device frame of the handle's geometry, read in place at its own pitch; prev, cur and
+ * next may be the same frame (the ends of a clip).  The kernel orders itself behind the sources' producers and the
+ * outputs' previous readers and is recorded as a reader of the sources and the producer of the outputs; nothing waits
+ * on the host.  A host frame reaches the handle through hbcu_xfer_upload once, however many pictures read it. */
+int  hbcu_deint_frame(hbcu_deint_t *h, hbcu_frame_t *prev, hbcu_frame_t *cur, hbcu_frame_t *next, int tff, int spatial,
+                      int npictures, hbcu_frame_t *const out[2], const int parity[2], const int intra[2]);
+int  hbcu_deint_sync(hbcu_deint_t *h);
+int  hbcu_deint_mark(hbcu_deint_t *h, int which);
+int  hbcu_deint_elapsed_ms(hbcu_deint_t *h, float *ms);
+
 #ifdef __cplusplus
 }
 #endif
